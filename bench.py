@@ -1,11 +1,15 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the depth hot path (BASELINE.json metric: BAM GB/s for `depth base`).
+"""bench.py -- headline benchmark of the depth hot path (BAM GB/s for `depth base`).
 
   python bench.py --gpus N --steps K --warmup W            # our arm (libbdepth.so through the C ABI)
   python bench.py --impl reference --gpus N --steps K ...  # reference arm: the CPU implementation on host cores
+  python bench.py ... --dump-outputs DIR                   # also write what the last timed end-to-end step delivered (.npy)
+
+It runs from the tree as build() left it and writes nothing there: the workload is generated into BDEPTH_BENCH_DIR
+(default: a directory under the system's temporary directory).
 
 Workload (config.workload): BASELINE configs[1], the synthetic 30x chr20 BAM (64,444,167 bp, 12,888,833 x 150 bp
-reads, seed 20, zlib level 6, 0xFF00-byte BGZF blocks) generated on the box by tools/bamgen.c.  At N > 1 GPUs
+reads, seed 20, zlib level 6, 0xFF00-byte BGZF blocks) generated on first use by tools/bamgen.c.  At N > 1 GPUs
 the input grows with N (N chromosomes of that size, weak scaling, the shape of BASELINE configs[3]) and is sharded
 by BGZF virtual offset at BAI linear-index record starts; boundary counters are exchanged over NCCL.
 
@@ -15,7 +19,7 @@ A "step" is one complete `depth base` pass over the whole input:
   e2e    : bdepth_open_memory() on the BAM image in PINNED HOST memory + bdepth_run_base(): H2D of the compressed
            bytes, all kernels, and D2H of the 7 x u32 per-position counters into pinned host memory, all inside
            the timed region (host wall clock around the call, which ends in a stream synchronize).
-The file is 2.26 GB compressed / 3.76 GB inflated per chromosome unit, far larger than the 126 MB L2, so no L2
+The file is 2.26 GB compressed / 3.76 GB inflated per chromosome unit, far larger than an H100's 50 MB L2, so no L2
 flush is needed between steps (config.l2: "inputs >> L2").
 """
 import argparse
@@ -26,9 +30,11 @@ import os
 import shutil
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
+sys.dont_write_bytecode = True          # the tree may be read-only: no __pycache__ from the imports below
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -40,45 +46,32 @@ READS_PER_UNIT = 12888833
 UNIT_LEN = int(os.environ.get("BDEPTH_BENCH_UNIT_LEN", "64444167"))      # (the override is for tests/run_bench_emul.py: the CPU emulation cannot sweep 64 Mbp in a test's time)
 
 
-def ncu_traffic(kernel_key):
-    """roofline.traffic = dram__bytes_read.sum + dram__bytes_write.sum per launch of the kernel, parsed from the ncu
-    summary profiles/CURRENT.json names for it (the capture of the shipped build; tools/ncu_summary.py wrote it)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "CURRENT.json")) as f:
-            ent = json.load(f)[kernel_key]
-        tot, inside = 0.0, False
-        with open(os.path.join(ROOT, ent["summary"])) as f:
-            for line in f:
-                if line.startswith("== kernel:"):
-                    inside = any(m in line for m in ent["kernel_match"])        # the K1 stage is two launches (k1_huff, k1_lz): their traffic adds
-                elif inside and ("dram__bytes_read.sum" in line or "dram__bytes_write.sum" in line):
-                    unit = line.split("[")[1].split("]")[0].lower()
-                    v = float(line.rsplit("=", 1)[1].replace(",", ""))
-                    tot += v * {"gbyte": 1e9, "mbyte": 1e6, "kbyte": 1e3, "byte": 1.0, "tbyte": 1e12}[unit]
-                elif inside and line.startswith("== hottest"):
-                    inside = False
-        return (int(tot) if tot else None), ent["summary"]
-    except Exception as e:                                    # no capture of this build yet: say so instead of quoting a stale one
-        return None, f"none ({type(e).__name__})"
-
-
 def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return json.load(f)["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs, copy bandwidth)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM, 3.35 TB/s HBM3); not a measured rate"
+
+
+def bench_dir():
+    d = os.environ.get("BDEPTH_BENCH_DIR") or os.path.join(tempfile.gettempdir(), "bdepth_bench")
+    os.makedirs(d, exist_ok=True)
+    return d
+
+
+def require_build(load=True):
+    """The generator and the checker that build() compiled; load=True also maps the product library (the reference arm never does)."""
+    for exe in (os.path.join(ROOT, "tools", "_build", "bamgen"), os.path.join(ROOT, "oracle", "_build", "depth_oracle")):
+        if not os.path.exists(exe):
+            raise SystemExit(f"bench.py: {exe} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` first")
+    if load:
+        import sambamba_b200
+        sambamba_b200.load_library()
 
 
 def workload_path(n_units, reads_per_unit):
-    d = os.environ.get("BDEPTH_BENCH_DIR", "/tmp/bdepth_bench")
-    os.makedirs(d, exist_ok=True)
-    return os.path.join(d, f"synth_chr20x{n_units}_{reads_per_unit}" + ("" if UNIT_LEN == 64444167 else f"_len{UNIT_LEN}") + ".bam")
+    return os.path.join(bench_dir(), f"synth_chr20x{n_units}_{reads_per_unit}" + ("" if UNIT_LEN == 64444167 else f"_len{UNIT_LEN}") + ".bam")
 
 
 def ensure_workload(n_units, reads_per_unit, load=True):
-    import __graft_entry__ as g
-    g.build(quiet=True, load=load)          # load=False (reference arm): the product library is never mapped into that process
+    require_build(load)          # load=False (reference arm): the product library is never mapped into that process
     path = workload_path(n_units, reads_per_unit)
     if os.path.exists(path) and os.path.exists(path + ".bai"):
         return path
@@ -107,13 +100,11 @@ def wgs_refs(scale=None):
 
 def ensure_wgs(load=True):
     """BASELINE configs[2..4] input: the 24 GRCh38 primary chromosomes, 30x of 150 bp reads, seed 30 (SURVEY 8d) -- at 1 / WGS_SCALE
-    linear scale: a full-size one is 108 GB of BAM, more than the box's 79 GB disk and ~10 minutes of generation per bench run.
+    linear scale: a full-size one is 108 GB of BAM, more disk than a bench run should assume and ~10 minutes of generation.
     Every per-position ratio (reads per tile, bytes per position, blocks per Mbp) is that of the full genome; 62 M reads,
     10.8 GB of BAM, 18 GB inflated = three 6 GiB HBM batches, so the carry / tile-window / prefetch paths are all in the timing."""
-    import __graft_entry__ as g
-    g.build(quiet=True, load=load)
-    d = os.environ.get("BDEPTH_BENCH_DIR", "/tmp/bdepth_bench")
-    os.makedirs(d, exist_ok=True)
+    require_build(load)
+    d = bench_dir()
     n = WGS_READS // WGS_SCALE
     path = os.path.join(d, f"synth_wgs_div{WGS_SCALE}_{n}.bam")
     if os.path.exists(path) and os.path.exists(path + ".bai"):
@@ -148,7 +139,7 @@ def exome_bed(refs, n_total, seed=50):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
 
     def __init__(self, gpu_index):
         self.rows = []
@@ -272,6 +263,32 @@ def checksum_run(h, lin0):
     return acc
 
 
+DUMP_POSITIONS = 1 << 20          # --dump-outputs: 7 x 2^20 float32 counters + 2^20 float64 positions = 36 MB
+
+
+def dump_sampler(h, seed=20):
+    """A tile callback that keeps the 7 counters (A, C, G, T, N, DEL, REFSKIP) of a fixed, seeded sample of linear positions
+    (all of them when the genome is that short): returns (callback, positions, counts[7, n])."""
+    import numpy as np
+    import sambamba_b200._lib as L
+    lin0 = np.concatenate([[0], np.cumsum([l for _, l in h.refs])]).astype(np.int64)
+    total = int(lin0[-1])
+    pos = np.arange(total, dtype=np.int64) if total <= DUMP_POSITIONS else np.sort(np.random.default_rng(seed).choice(total, DUMP_POSITIONS, replace=False))
+    counts = np.zeros((7, len(pos)), np.float32)
+
+    def cb(_user, tp):
+        t = tp.contents
+        a = int(lin0[t.ref_id]) + t.start
+        lo, hi = np.searchsorted(pos, [a, a + t.len])
+        if hi > lo:
+            src = np.ctypeslib.as_array(t.counts, shape=(6 * t.stride + t.len,))
+            off = pos[lo:hi] - a
+            for p in range(7):
+                counts[p, lo:hi] = src[p * t.stride + off]
+        return 0
+    return L.TILE_CB(cb), pos, counts
+
+
 def oracle_checksums(path, threads):
     """The same three numbers from the CPU oracle's closed-form counters over the whole genome (test infrastructure; the
     only use of oracle/ in our arm is this check AFTER the timed region)."""
@@ -288,9 +305,9 @@ def oracle_checksums(path, threads):
 
 
 T_PROCESS_START = time.time()
-# The driver gives one bench launch 870 s (SCALE_r01.json per_n_timeout_s).  The oracle's whole-file closed form is the one leg whose duration grows
-# with N (about 30 s per chr20 unit on 64 host threads): it runs under a deadline, and a run that cannot finish the check in time still prints
-# its line -- with "verified": null and the reason -- instead of being killed without one.
+# A bench run is commonly given a fixed time budget (BDEPTH_BENCH_BUDGET_S).  The oracle's whole-file closed form is the one leg whose duration
+# grows with N (about 30 s per chr20 unit on 64 host threads): it runs under a deadline, and a run that cannot finish the check in time still
+# prints its line -- with "verified": null and the reason -- instead of being killed without one.
 BENCH_BUDGET_S = float(os.environ.get("BDEPTH_BENCH_BUDGET_S", "780"))
 
 
@@ -511,7 +528,6 @@ def run_wgs_config(a, rank, world, local_rank):
             dist.destroy_process_group()
         return 0
     peak, peak_src = peaks()
-    traffic, traffic_src = ncu_traffic("roofline")
     value = file_bytes / 1e9 / (ms_step / 1e3)
     out = {
         "metric": metric, "value": value, "unit": "GB/s", "n_gpus": a.gpus, "steps": a.steps, "warmup": a.warmup, "ms_per_step": ms_step, "higher_is_better": True,
@@ -524,7 +540,7 @@ def run_wgs_config(a, rank, world, local_rank):
                 "path": "bdepth_open_memory(pinned host BAM image) + " + {"window": "bdepth_run_windows", "wgs-shard": "bdepth_run_base", "exome": "bdepth_run_regions"}[a.config], "host_input": host_kind},
         "gpu_launches": int(total_launches),
         "roofline": {"kernel": "K1 two-phase inflate (k1_huff + k1_lz)", "bound": "hbm", "achieved": k1_bytes / 1e9 / (k1_ms / 1e3) if k1_ms else None, "peak": peak, "unit": "GB/s",
-                     "frac": (k1_bytes / 1e9 / (k1_ms / 1e3) / peak) if k1_ms else None, "traffic": None, "traffic_source": "per-launch capture exists for the chr20 workload only (" + str(traffic_src) + ")",
+                     "frac": (k1_bytes / 1e9 / (k1_ms / 1e3) / peak) if k1_ms else None, "traffic": None, "traffic_source": "not measured",
                      "algorithmic_bytes_per_launch": int(k1_bytes / max(1, n_batches)), "launches_per_step": n_batches, "peak_source": peak_src,
                      "note": "C + U of this rank's shard / CUDA-event time of its K1 launches"},
         "clocks": clocks, "verified": (verify["ok"] if verify else None), "verification": verify,
@@ -569,7 +585,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-full-file", action="store_true", help="reference arm: skip the one whole-file run of the port")
     ap.add_argument("--no-verify", action="store_true", help="development only: skip the bit-exact check of the counters after the timed region")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed end-to-end step delivered to DIR as .npy (chr20 config): "
+                    "positions.npy (a fixed, seeded sample of linear positions), counts.npy (their 7 counters), resident_stats.npy")
     a = ap.parse_args()
+    if a.dump_outputs and (a.config != "chr20" or a.impl != "ours"):
+        ap.error("--dump-outputs is for the GPU arm of the chr20 config")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -695,12 +715,13 @@ def main():
     st = b.stats()
     ms_step = sum(span) / len(span)
     covered = sum_over_ranks(st["covered_positions"])
+    resident_stats = [sum_over_ranks(st["n_records"]), sum_over_ranks(st["n_records_pass"]), covered]      # what bdepth_run_resident's caller receives
     total_launches = sum_over_ranks(launches)
     k1_ms = sum(k1) / len(k1)
     k1_bytes = st["cdata_bytes"] + st["inflated_bytes"]              # C + U of this rank's shard (SURVEY 8d)
     k1_launches_per_step = st["n_batches"]
     # ---- A/B on the same resident handle (one GPU only; the library reads its switches at every run): kernels this build replaced,
-    # measured beside the shipped ones so that a change made without access to a GPU shows its effect in the line the driver records
+    # measured beside the shipped ones so that a change made without access to a GPU shows its effect in the line bench.py prints
     ab = None
     if world == 1:
         ab = {"what": "stage times (ms) of 3 resident passes with one library switch each, same handle and input as `value`",
@@ -740,10 +761,14 @@ def main():
     open_s = time.perf_counter() - t0
     cold_s = None
     n_w = max(1, min(a.warmup, 3))
+    dump = dump_sampler(h) if a.dump_outputs else None
     for i in range(n_w + a.steps):
         barrier()
         t0 = time.perf_counter()
-        h.run_base(collect=False)                                   # H2D of the compressed bytes + kernels + D2H of the counters
+        if dump is not None and i == n_w + a.steps - 1:
+            h._ck(h.L.bdepth_run_base(h.h, dump[0], None))         # the last timed step also hands its tiles to the sampler
+        else:
+            h.run_base(collect=False)                               # H2D of the compressed bytes + kernels + D2H of the counters
         dt = time.perf_counter() - t0
         s2 = h.stats()
         d2h_bytes = (s2["own_hi"] - s2["own_lo"]) * 28
@@ -802,6 +827,18 @@ def main():
                       "covered_positions": got[2], "oracle_covered_positions": want[2], "positions_delivered": got[3], "oracle_seconds": time.perf_counter() - t0,
                       "what": "sum over planes p, positions g of count*((g*A+(p+1)*B)|1) mod 2^64 over every rank's delivered tiles vs the CPU oracle's closed-form counters of the whole file"}
     h.close()
+    if dump is not None:
+        _, dump_pos, dump_counts = dump
+        if dist is not None:                 # every rank delivered its own positions (disjoint): the sum is the whole sample
+            import torch
+            t = torch.from_numpy(dump_counts).cuda()
+            dist.all_reduce(t, op=dist.ReduceOp.SUM)
+            dump_counts = t.cpu().numpy()
+        if rank == 0:
+            os.makedirs(a.dump_outputs, exist_ok=True)
+            np.save(os.path.join(a.dump_outputs, "positions.npy"), dump_pos.astype(np.float64))
+            np.save(os.path.join(a.dump_outputs, "counts.npy"), dump_counts)
+            np.save(os.path.join(a.dump_outputs, "resident_stats.npy"), np.array(resident_stats, np.float64))
     e2e_s = sum(e2e_t) / len(e2e_t)
     h2d_total = file_bytes
     d2h_total = sum_over_ranks(d2h_bytes)
@@ -811,7 +848,6 @@ def main():
             dist.destroy_process_group()
         return 0
     peak, peak_src = peaks()
-    traffic, traffic_src = ncu_traffic("roofline")
     value = file_bytes / 1e9 / (ms_step / 1e3)
     out = {
         "metric": "bam_gb_per_s_depth_base", "value": value, "unit": "GB/s", "n_gpus": a.gpus, "steps": a.steps, "warmup": a.warmup,
@@ -827,7 +863,7 @@ def main():
         "text_rows": text, "ab": ab,
         "gpu_launches": int(total_launches),
         "roofline": {"kernel": "K1 two-phase inflate: k1_huff (lane-per-BGZF-block Huffman phase) + k1_lz (warp-per-block LZ77 phase), timed together", "bound": "hbm", "achieved": k1_bytes / 1e9 / (k1_ms / 1e3), "peak": peak, "unit": "GB/s",
-                     "frac": k1_bytes / 1e9 / (k1_ms / 1e3) / peak, "traffic": traffic if (a.gpus == 1 and a.reads_per_unit == READS_PER_UNIT) else None, "traffic_source": traffic_src,
+                     "frac": k1_bytes / 1e9 / (k1_ms / 1e3) / peak, "traffic": None, "traffic_source": "not measured",
                      "algorithmic_bytes_per_launch": int(k1_bytes / max(1, k1_launches_per_step)), "launches_per_step": k1_launches_per_step,
                      "peak_source": peak_src, "note": "C + U per pass (SURVEY 8d) / CUDA-event duration of the K1 launches (k1_huff + k1_lz + k1_fallback) on the library stream; phase 1 is instruction-latency bound, phase 2 issue bound, neither HBM bound"},
         "clocks": clocks,

@@ -1,5 +1,5 @@
 /*
- * bdepth.h -- C ABI of libbdepth.so, the B200-native engine behind `sambamba depth`.
+ * bdepth.h -- C ABI of libbdepth.so, the H100-native engine behind `sambamba depth`.
  *
  * The reference has NO foreign-function boundary on this path (SURVEY.md F4): `depth` is D
  * ranges composed in one function, sambamba/depth.d:1211-1232.  This header therefore DEFINES

@@ -9,7 +9,7 @@
  * The reference (biod/sambamba @ v1.0.1) is D and cannot be compiled in this
  * image (no ldc2/dmd/gdc), so this is a "port" oracle.  It is pinned against
  * the reference's own golden files (tests/golden/, copied from
- * /root/reference/test/): issue_193, issue225 (-c 1 / -c 0, with and without
+ * the reference's test/ directory): issue_193, issue225 (-c 1 / -c 0, with and without
  * -L chrM) and issue_204 (region -T x3 -m).  See tests/test_oracle_golden.py.
  *
  * Third-party arithmetic: raw DEFLATE inflate lives in system zlib, exactly as
@@ -18,7 +18,7 @@
  * library.
  *
  * Each section cites the reference file:line it follows (paths relative to
- * /root/reference).  Nothing here is copied from the reference; it is C
+ * biod/sambamba v1.0.1).  Nothing here is copied from the reference; it is C
  * restating D semantics.
  *
  * Build:  make -C oracle     (-> oracle/_build/depth_oracle, liboracle.so)

@@ -1,4 +1,4 @@
-"""sambamba_b200 -- B200-native engine behind `sambamba depth` (see DESIGN.md).
+"""sambamba_b200 -- H100-native (sm_90a) engine behind `sambamba depth` (see DESIGN.md).
 
 Python is only the test/bench harness around libbdepth.so (the C ABI in include/bdepth.h);
 the product is the CUDA library and the C++ CLI host in sambamba_b200/csrc.

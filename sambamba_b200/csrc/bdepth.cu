@@ -141,7 +141,7 @@ struct bdepth {
     // needs them all; a region query never does (plan_sparse frames the members of its BAI chunks on its own)
     bool lazy = false, framed_all = true; size_t framed_off = 0;
     BamHeader hdr; BaiIndex bai; bool has_index = false;
-    int device = 0;
+    int device = 0; int n_sm = 0;       // SM count of the device (K1 launch-shape choice)
     // ---- config
     int mapq_gt = 0; uint32_t flag_reject = 0x600; uint32_t minq = 0;
     std::vector<bdepth_region> regions;   // merged, sorted
@@ -235,6 +235,7 @@ int init_device(bdepth* h) {
     if (e != cudaSuccess || n <= 0) return fail(h, BDEPTH_ERR_CUDA, "no CUDA device available (%s); libbdepth has no CPU fallback", cudaGetErrorString(e));
     if (h->device < 0 || h->device >= n) return fail(h, BDEPTH_ERR_ARG, "device %d out of range (%d devices)", h->device, n);
     CK(cudaSetDevice(h->device));
+    CK(cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, h->device));
     if (!h->s_main) { CK(cudaStreamCreateWithFlags(&h->s_main, cudaStreamNonBlocking)); CK(cudaStreamCreateWithFlags(&h->s_copy, cudaStreamNonBlocking)); CK(cudaStreamCreateWithFlags(&h->s_d2h, cudaStreamNonBlocking)); for (auto& ks : h->s_k1) CK(cudaStreamCreateWithFlags(&ks, cudaStreamNonBlocking)); for (auto& e2 : h->ev) CK(cudaEventCreate(&e2)); }
     CK(cudaFuncSetAttribute(k1_inflate, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM));
     CK(cudaFuncSetAttribute(k1_fallback, cudaFuncAttributeMaxDynamicSharedMemorySize, K1_SMEM));
@@ -245,7 +246,7 @@ int init_device(bdepth* h) {
     CK(cudaFuncSetAttribute(k3_tile<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K3T_SMEM)); CK(cudaFuncSetAttribute(k3_tile<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K3T_SMEM));
     { const char* e = getenv("BDEPTH_K1LZ"); h->k1lz_flat = e && !strcmp(e, "flat"); h->k1lz_v12 = e && !strcmp(e, "v12"); }      // A/B of the two phase-2 kernels
     { const char* e = getenv("BDEPTH_K1_ONEPHASE"); h->k1_onephase = e && atoi(e) == 1; }
-    { const char* e = getenv("BDEPTH_K3_PREFETCH"); h->k3_pre = !e || atoi(e) != 0; }      // default since round 2: measured 10.4 -> 8.4 ms on chr20 (profiles/k3_history.md)
+    { const char* e = getenv("BDEPTH_K3_PREFETCH"); h->k3_pre = !e || atoi(e) != 0; }      // default: k3_gather prefetches the records of its tile lane-parallel
     return 0;
 }
 
@@ -653,7 +654,8 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     cudaStream_t sm = h->s_main;
 
     // ---- counter window (28 B/position).  With a BAI the linear index bounds where reads can lie, so only that
-    // span of the linear genome is allocated; without one the whole genome is (87 GB for GRCh38, fits 180 GB HBM).
+    // span of the linear genome is allocated; without one the whole genome is (87 GB for GRCh38: more than an 80 GB H100 holds, so
+    // such a run ends with the BDEPTH_ERR_CUDA below instead of starting).
     if (mode == RUN_FULL && h->accum) {
         // a further input of the same run: counters, window, sample planes stay as the first input left them
     } else if (mode == RUN_FULL) {
@@ -858,8 +860,8 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             const unsigned hg = (n + 32 * K1H_WARPS - 1) / (32 * K1H_WARPS); const uint32_t blk0 = (uint32_t)(c0 - b);
 #define K1H(LIMS, MINB) BD_LAUNCH(hg, 32 * K1H_WARPS, k1h_smem<LIMS>(), ks, k1_huff<LIMS, MINB>)(d_comp, dd, n, blk0, stp, h->tok.as<uint32_t>(), h->lits.as<uint8_t>(), ax, sgi, ltb)
             // which instantiation: limits in registers at 4 CTAs per SM (16 warps) is the faster loop; when a launch has more warps than that
-            // holds at once, limits in shared memory at 5 CTAs (20 warps) wins by its occupancy (profiles/k1_history.md)
-            const int variant = h->k1h_variant >= 0 ? h->k1h_variant : (n > 148u * 16u * 32u ? 2 : 0);
+            // holds at once (16 warps on every SM of the device), limits in shared memory at 5 CTAs (20 warps) wins by its occupancy
+            const int variant = h->k1h_variant >= 0 ? h->k1h_variant : (n > (uint32_t)h->n_sm * 16u * 32u ? 2 : 0);
             switch (variant) { case 1: K1H(false, 6); break; case 2: K1H(true, 5); break; case 3: K1H(true, 4); break; default: K1H(false, 4); }
 #undef K1H
             if (h->k1lz_flat) BD_LAUNCH((n + K1L_WARPS - 1) / K1L_WARPS, 32 * K1L_WARPS, 0, ks, k1_lz_flat)(dd, n, blk0, u0, stp, h->tok.as<uint32_t>(), h->lits.as<uint8_t>(), ax, sgi, ltb);

@@ -2,7 +2,7 @@
 // zlib inflate, bound in BioD/bio/core/utils/zlib.d:143-162); RFC 1951 output is deterministic, so the result is
 // bit-identical to zlib's whatever the decomposition.
 //
-// Why two phases (profiles/r1_k1_v8_two_literal_ncu_full_summary.txt): the one-phase lane-per-block decoder
+// Why two phases: the one-phase lane-per-block decoder
 // (inflate_core.cuh, kept as the exact fallback and for the header blocks) executes the union of "decode a symbol",
 // "append bytes", "fetch a round of an LZ77 copy" for 32 lanes in different states -- 535 instructions per iteration at
 // 15 of 32 active lanes -- and every far LZ77 source is a DRAM sector of one of 57 k concurrent 32 KB windows

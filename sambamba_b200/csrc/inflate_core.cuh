@@ -3,7 +3,7 @@
 //
 // Replaces: BioD/bio/core/bgzf/block.d:127-216 (decompressBgzfBlock -> zlib inflateInit2(-15)/
 // inflate(Z_FINISH)/inflateEnd, bound through BioD/bio/core/utils/zlib.d:143-162).  The
-// arithmetic being restated is zlib's (third-party, not under /root/reference); RFC 1951 output
+// arithmetic being restated is zlib's (third-party, not in the sambamba sources); RFC 1951 output
 // is deterministic so any correct inflater is bit-identical.
 //
 // Design (see DESIGN.md "K1").  A warp-per-block decoder issues ~200 instructions per symbol
@@ -84,7 +84,7 @@ constexpr uint32_t NEAR_MAX = 4 * (RING_WORDS - 1) - 4;   // 24: farthest distan
 // Ampere-style asynchronous copies (LDGSTS).  Their completion is tracked by cp.async groups, NOT by the register
 // scoreboard, so a copy issued at the end of one loop iteration is still in flight at the top of the next; plain
 // loads whose result crosses the loop back-edge are waited for at the back-edge by the compiler (that wait was
-// 30 % of all stall samples in profiles/r1_k1_inflate_ncu_full_summary.txt).
+// the largest single stall reason of the one-phase decoder's loop).
 __device__ __forceinline__ void cp_async16(uint32_t saddr, const void* g) { asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(saddr), "l"(g) : "memory"); }
 __device__ __forceinline__ void cp_async4(uint32_t saddr, const void* g) { asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" :: "r"(saddr), "l"(g) : "memory"); }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
@@ -401,7 +401,7 @@ enum { ST_HDR = 0, ST_SYM = 1, ST_STORED = 2, ST_DONE = 3 };
 // Warp convergence.  Lanes take different paths through an iteration (literal / match / header)
 // and finish their blocks at different times.  With independent thread scheduling nothing forces
 // them back together, and the first version of this kernel ran with 1.02 active threads per
-// instruction (ncu, profiles/k1_v1_summary.md).  Every iteration therefore ends in a ballot over
+// instruction.  Every iteration therefore ends in a ballot over
 // the lanes still decoding: it is both the reconvergence point and the next iteration's mask.
 #if defined(__CUDA_ARCH__)
 #define BD_BALLOT(mask, pred) __ballot_sync((mask), (pred))

@@ -1,4 +1,4 @@
-// kernels.cuh -- the sm_100a kernels of the depth hot path.
+// kernels.cuh -- the sm_90a kernels of the depth hot path.
 //
 //   K1  k1_inflate          lane-per-BGZF-block DEFLATE (inflate_core.cuh)
 //   K2  k2_guess_entries    first record start of every BGZF block (speculative, verified)
@@ -12,7 +12,7 @@
 //   R   k_tile_covered, k_bucket_stats, k_read_windows, k_read_regions : reducers for the
 //       base / window / region front ends
 //
-// Semantics restated (file:line under /root/reference):
+// Semantics restated (file:line in the biod/sambamba v1.0.1 sources):
 //   record layout      BioD/bio/std/hts/bam/read.d:907-1003, readrange.d:118-173
 //   CIGAR predicates   BioD/bio/std/hts/bam/cigar.d:58-148 (CIGAR_TYPE :116)
 //   filter             sambamba/depth.d:1159, filtering.d:163-167,194-214
@@ -51,10 +51,9 @@ struct BlockAux { uint32_t n_tok, n_seg, n_lit, pad; };      // what phase 1 fou
 // Literal area of block i of a batch (16-byte aligned, >= isize bytes, disjoint from its neighbours'): derived from the output offset.
 BD_HD uint64_t lit_off_of(uint64_t uoff, uint64_t block_index) { return (uoff & ~15ull) + 16ull * block_index; }
 
-// One CTA of 13 warps per SM: 13 x 17,664 B = 229,632 B of dynamic shared memory (the per-CTA 1 KB system
-// reservation is paid once, which is what lets a 13th warp fit).  148 x 13 x 32 = 61,568 BGZF blocks in flight:
-// a 30x chromosome (57.6 k blocks) is a single wave with no tail (12 one-warp CTAs per SM left 5 warps for a
-// second wave that cost 35 % of the kernel time, profiles/k1_history.md).
+// One CTA of 13 warps per SM: 13 x 17,664 B = 229,632 B of dynamic shared memory, within the 227 KB a CTA may have on
+// sm_90 (the per-CTA 1 KB system reservation is paid once, which is what lets a 13th warp fit).  This kernel only inflates
+// the header blocks and the blocks the two-phase inflater hands back, so its shape is set by shared memory, not by the SM count.
 constexpr int K1_WARPS = 13;
 constexpr int K1_SMEM = K1_WARPS * SMEM_BYTES_PER_WARP;         // 229,632 B
 __global__ void __launch_bounds__(K1_WARPS * 32, 1) k1_inflate(const uint32_t* __restrict__ comp, const BlockDesc* __restrict__ blocks,
@@ -79,7 +78,7 @@ __global__ void __launch_bounds__(K1_WARPS * 32, 1) k1_inflate(const uint32_t* _
 constexpr int K1H_WARPS = 4;
 template <bool LIMS> constexpr int k1h_smem() { return K1H_WARPS * (H_SMEM_BYTES_PER_WARP + (LIMS ? H_LIM_BYTES_PER_WARP : 0)); }      // 32 KB / 40 KB
 // LIMS / MINB: where the Huffman limits live and how many CTAs per SM the register allocation aims at -- the variants
-// measured against each other in profiles/k1_history.md.  blk0: index of blocks[0] in the batch (literal areas are per batch).
+// selected in bdepth.cu by launch size.  blk0: index of blocks[0] in the batch (literal areas are per batch).
 template <bool LIMS, int MINB>
 __global__ void __launch_bounds__(K1H_WARPS * 32, MINB) k1_huff(const uint32_t* __restrict__ comp, const BlockDesc* __restrict__ blocks, uint32_t n_blocks, uint32_t blk0,
                                                                 int* __restrict__ status, uint32_t* __restrict__ tok, uint8_t* __restrict__ lits, BlockAux* __restrict__ aux,
@@ -179,7 +178,7 @@ __global__ void __launch_bounds__(K1L_WARPS * 32, 6) k1_lz(const BlockDesc* __re
             // lanes stride over the packed ranks four at a time (one unaligned word per lane and round: a group's ~130 literals are one
             // round); the token a literal belongs to is found by a binary search over the 32 inclusive counts in shared memory for the
             // first of the four and by stepping for the others; rank -> byte through the deflate block's table in shared memory
-            // (measured against a lane-per-token copy of the runs: 11.6 vs 12.9 ms, profiles/k1_history.md)
+            // (faster than a lane-per-token copy of the runs)
             // Only the tokens that have literals enter the table (compacted by a ballot): every entry then covers at least one literal, so
             // from one literal to the next the token changes by at most one entry -- one predicated step per byte instead of a loop over
             // the match-only tokens in between (that loop was 13 % of the kernel's instructions at 7 of 32 lanes).
@@ -363,7 +362,7 @@ __global__ void __launch_bounds__(K1_WARPS * 32, 1) k1_fallback(const uint32_t* 
 
 // ------------------------------------------------------------------------------------- K2
 // Unaligned little-endian loads from the inflated stream: two aligned 32-bit loads + funnel shift (records are
-// byte-aligned; four byte loads per field made k2_decode LSU-queue bound: profiles/r1_k2_k3_ncu_full_summary.txt).
+// byte-aligned; four byte loads per field make k2_decode LSU-queue bound).
 // The buffer has >= 256 readable bytes after its end, so touching the following word is always legal.
 __device__ __forceinline__ uint32_t ldu32(const uint8_t* p) {
     uintptr_t a = reinterpret_cast<uintptr_t>(p);
@@ -681,8 +680,8 @@ __device__ __forceinline__ void add_base(GatherAcc& a, int j, const uint8_t* seq
 // PRE (EXPERIMENT, off by default, BDEPTH_K3_PREFETCH=1): the lane that holds candidate read base+i also loads that
 // read's off / ncl / lseq / first CIGAR word, 32 reads per load instruction, and the per-read step takes them by
 // shuffle.  Without it every selected read costs a chain of four dependent global loads (off -> ncl/lseq -> CIGAR
-// word -> sequence bytes) that all 32 lanes wait for: ~56 reads per warp x ~2 us; the kernel's 7.4 ms is about what
-// that latency chain predicts at 32 resident warps per SM.  Never measured: DESIGN.md section 10.
+// word -> sequence bytes) that all 32 lanes wait for: ~56 reads per warp x ~2 us, which is
+// what bounds the kernel at 32 resident warps per SM.
 template <bool MINQ, bool PRE>
 __global__ void __launch_bounds__(256) k3_gather(RecordSoA soa, const uint8_t* __restrict__ u, uint64_t tiles_base, uint64_t cnt_base, uint64_t win_len,
                                                   const uint32_t* __restrict__ tile_first, const uint32_t* __restrict__ tile_lo,

@@ -131,6 +131,8 @@ static inline cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t) { e->t = 
 static inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess; }
 static inline cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t a, cudaEvent_t b) { *ms = (float)(b->t - a->t); return cudaSuccess; }
 template <class F> static inline cudaError_t cudaFuncSetAttribute(F, int, int) { return cudaSuccess; }
+enum { cudaDevAttrMultiProcessorCount = 16 };
+static inline cudaError_t cudaDeviceGetAttribute(int* v, int, int) { *v = 132; return cudaSuccess; }      // an H100 SXM's SM count
 
 // ------------------------------------------------------------------------------------------------ NCCL stand-in
 // Ranks are THREADS of one process under emulation (the tests start one thread per rank; ctypes releases the GIL).  The

@@ -145,7 +145,7 @@ def test_region_chunk_plan_covers_every_overlapping_record(tmp_path):
 
 
 def test_bench_reference_arm_prints_its_line(tmp_path):
-    """`bench.py --impl reference` (the CPU arm the driver times beside the GPU one) on a small workload: one JSON line with
+    """`bench.py --impl reference` (the CPU arm timed beside the GPU one) on a small workload: one JSON line with
     the contract's keys, measured on a bounded sample that ends mid-stream (the oracle tolerates the cut only there)."""
     import json
     import subprocess
@@ -165,13 +165,14 @@ def test_bench_reference_arm_prints_its_line(tmp_path):
 def test_bench_own_arm_control_flow_under_the_emulation(tmp_path):
     """bench.py's own arm with the product library replaced by its CUDA-on-CPU emulation build (tests/run_bench_emul.py): warm-up, timed
     passes, the A/B legs, e2e, text rows and the verification against the oracle all run and the line carries the contract's keys.
-    (What the numbers are is meaningless here; that the round-end launch cannot die of a Python error is the point.)"""
+    (What the numbers are is meaningless here; that a GPU run of bench.py cannot die of a Python error is the point.)"""
     import json
     import subprocess
     import sys
     env = dict(os.environ, BDEPTH_BENCH_DIR=str(tmp_path), BDEPTH_BENCH_UNIT_LEN="300000")
-    r = subprocess.run([sys.executable, os.path.join(helpers.ROOT, "tests", "run_bench_emul.py"), "--reads-per-unit", "15000", "--steps", "1", "--warmup", "1", "--cpu-sample-mb", "1"],
-                       capture_output=True, text=True, env=env, timeout=900)
+    dump = tmp_path / "dump"
+    r = subprocess.run([sys.executable, os.path.join(helpers.ROOT, "tests", "run_bench_emul.py"), "--reads-per-unit", "15000", "--steps", "1", "--warmup", "1", "--cpu-sample-mb", "1",
+                        "--dump-outputs", str(dump)], capture_output=True, text=True, env=env, timeout=900)
     assert r.returncode == 0, r.stderr[-600:]
     line = json.loads(r.stdout.strip().splitlines()[-1])
     assert line["verified"] is True and line["verification"]["checksum"] == line["verification"]["oracle_checksum"]
@@ -180,6 +181,13 @@ def test_bench_own_arm_control_flow_under_the_emulation(tmp_path):
     assert line["e2e"]["h2d_bytes_per_step"] > 0 and line["e2e"]["d2h_bytes_per_step"] == 300000 * 28
     assert all("error" not in v for k, v in line["ab"].items() if isinstance(v, dict)), line["ab"]
     assert line["text_rows"]["text_bytes"] > 0
+    # --dump-outputs: the counters the last timed step delivered, at every position of this short genome, equal the oracle's
+    import numpy as np
+    pos, counts, res = (np.load(dump / f) for f in ("positions.npy", "counts.npy", "resident_stats.npy"))
+    assert pos.dtype == np.float64 and counts.dtype == np.float32 and res.dtype == np.float64
+    want, ost = helpers.oracle_counts(str(next(tmp_path.glob("*.bam"))))
+    assert np.array_equal(pos, np.arange(want.shape[1])) and np.array_equal(counts, want.astype(np.float32))
+    assert res.tolist() == [ost.n_records, ost.n_pass, ost.covered]
 
 
 def test_bench_verification_deadline():

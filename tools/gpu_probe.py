@@ -1,4 +1,4 @@
-"""Ad-hoc timing probe (run on the GPU box): per-stage device times from bdepth_stats."""
+"""Ad-hoc timing probe (needs a GPU): per-stage device times from bdepth_stats."""
 import os, sys, time, json, subprocess
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))

@@ -1,4 +1,4 @@
-"""Run `depth base` through the C ABI on a given (or generated) BAM: target for ncu captures.
+"""Run `depth base` through the C ABI on a given (or generated) BAM: a small target for profiler runs.
 usage: probe_one.py BAM [n_reads_if_missing] [reps] [--staged]"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
