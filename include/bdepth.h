@@ -20,6 +20,7 @@
  *     BGZF inflate   BioD/bio/core/bgzf/block.d:127-216                  bdepth_run_windows(PerWindowPrinter, depth.d:933-1077)
  *     record walk    BioD/bio/std/hts/bam/readrange.d:118-173            bdepth_run_regions(PerBedRegionPrinter, depth.d:879-931)
  *     column sweep   BioD/bio/std/hts/bam/pileup.d:345-424
+ *   computeFlagStatistics(bam.reads)     sambamba/flagstat.d:31-57,127   bdepth_run_flagstat (`sambamba flagstat`)
  *
  * Conventions: every entry returns 0 on success or a negative bdepth_status; the message is
  * available through bdepth_last_error().  No exception crosses the boundary.  There is no CPU
@@ -236,6 +237,20 @@ int64_t bdepth_inflate_to_host(bdepth_t* h, void* dst, uint64_t cap);
  * error.  The handle adopts the index: bdepth_has_index turns 1, and sharding, counter windows and region queries work on input
  * that came without a .bai (the reference refuses such input, depth.d:1166 -- the CLI still does unless --build-index is given). */
 int64_t bdepth_build_index(bdepth_t* h, void* dst, uint64_t cap);
+/* sambamba flagstat (flagstat.d:28-57): [0] QC-passed, [1] QC-failed (flag 0x200) */
+typedef struct { uint64_t total[2], secondary[2], supplementary[2], duplicates[2], mapped[2], paired[2], read1[2], read2[2],
+                 proper_pair[2], both_mapped[2], singletons[2], mate_diff_chr[2], mate_diff_chr_mapq5[2]; } bdepth_flagstat;
+/* The flag statistics `sambamba flagstat` prints: computeFlagStatistics (sambamba/flagstat.d:31-57), the loop flagstat_main runs over
+ * bam.reads (:119-128), as one call -- the options and the printing stay with the host (:99-150).  K1 inflate and the K2 record scan as
+ * in every run, then one thread per record (k_flagstat) with one ballot per category and warp.  Every record of the file is counted
+ * (all references and the unplaced tail); the file needs neither SO:coordinate nor a .bai on one GPU.  The handle's depth settings
+ * (filter, -F query, regions, -m, -q, --combined) do not apply and stay set for later runs.  Works on staged input and on
+ * bdepth_open_memory handles; a handle with bdepth_add_input files is BDEPTH_ERR_ARG (flagstat reads one file).  Several ranks:
+ * each counts the records of its shard (sharding needs the BAI) and one all-reduce sums them; without a NCCL id a rank returns its
+ * shard's counts.  Malformed input is BDEPTH_ERR_FORMAT as in every run -- which includes a record whose name, CIGAR, sequence and
+ * qualities overrun its block_size, a record the reference's release build would count.  Timings: ms_inflate, ms_scan and, for
+ * k_flagstat, ms_reduce of bdepth_stats. */
+int bdepth_run_flagstat(bdepth_t* h, bdepth_flagstat* out);
 /* Scan records on the GPU; copy out up to cap rows of the columnar SoA (any pointer may be NULL). */
 int64_t bdepth_scan_to_host(bdepth_t* h, uint64_t cap, int32_t* ref_id, int32_t* pos, uint32_t* span, uint16_t* flag, uint8_t* mapq, uint16_t* n_cigar, uint64_t* rec_off);
 

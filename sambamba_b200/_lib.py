@@ -46,6 +46,18 @@ class Stats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+FLAGSTAT_FIELDS = ("total", "secondary", "supplementary", "duplicates", "mapped", "paired", "read1", "read2", "proper_pair", "both_mapped",
+                   "singletons", "mate_diff_chr", "mate_diff_chr_mapq5")
+
+
+class FlagStat(C.Structure):
+    _fields_ = [(n, C.c_uint64 * 2) for n in FLAGSTAT_FIELDS]
+
+    def as_dict(self):
+        """{category: (QC-passed, QC-failed)} in the order of bdepth_flagstat."""
+        return {n: (getattr(self, n)[0], getattr(self, n)[1]) for n in FLAGSTAT_FIELDS}
+
+
 class TextOpts(C.Structure):
     _fields_ = [("min_cov", C.c_double), ("max_cov", C.c_double), ("annotate", C.c_int)]
 
@@ -114,6 +126,7 @@ def load_library():
     L.bdepth_scan_to_host.restype = C.c_int64
     L.bdepth_build_index.argtypes = [vp, vp, C.c_uint64]
     L.bdepth_build_index.restype = C.c_int64
+    L.bdepth_run_flagstat.argtypes = [vp, C.POINTER(FlagStat)]
     _lib = L
     return L
 
@@ -124,6 +137,7 @@ EXPORTED_SYMBOLS = [
     "bdepth_n_samples", "bdepth_sample_name", "bdepth_set_filter", "bdepth_set_filter_query", "bdepth_set_min_baseq", "bdepth_set_fix_mates", "bdepth_set_combined", "bdepth_set_regions",
     "bdepth_set_shard", "bdepth_nccl_unique_id", "bdepth_plan_shards", "bdepth_plan_region_chunks", "bdepth_set_tuning", "bdepth_stage", "bdepth_run_resident", "bdepth_run_base", "bdepth_run_base_text",
     "bdepth_run_windows", "bdepth_run_regions", "bdepth_get_stats", "bdepth_ref_has_reads", "bdepth_inflate_to_host", "bdepth_scan_to_host", "bdepth_build_index",
+    "bdepth_run_flagstat",
 ]
 
 
@@ -370,6 +384,12 @@ class BDepth:
         n2 = self._ck(self.L.bdepth_build_index(self.h, buf.ctypes.data_as(C.c_void_p), n))
         assert n2 == n
         return buf[:n].tobytes()
+
+    def run_flagstat(self):
+        """`sambamba flagstat` counters of the file (or shard): {category: (QC-passed, QC-failed)}."""
+        fs = FlagStat()
+        self._ck(self.L.bdepth_run_flagstat(self.h, C.byref(fs)))
+        return fs.as_dict()
 
     def scan(self, cap):
         cols = dict(ref_id=np.zeros(cap, np.int32), pos=np.zeros(cap, np.int32), span=np.zeros(cap, np.uint32),

@@ -80,7 +80,7 @@ constexpr size_t EMIT_CHUNK = 4ull << 20;     // positions per D2H chunk
 constexpr uint32_t SHARD_EXTRA_BLOCKS = 8;
 constexpr uint32_t MATE_ZONE_BLOCKS = 64;       // -m on several ranks: blocks read behind the shard so that pairs cut by the boundary are seen whole
 
-enum RunMode { RUN_FULL = 0, RUN_INFLATE_ONLY = 1, RUN_SCAN_ONLY = 2, RUN_INDEX = 3 };
+enum RunMode { RUN_FULL = 0, RUN_INFLATE_ONLY = 1, RUN_SCAN_ONLY = 2, RUN_INDEX = 3, RUN_FLAGSTAT = 4 };
 constexpr int RC_RETRY_WINDOW = 1;      // internal: a read lies outside the counter window a multi-input run was given
 
 // ---- NCCL, bound at run time (dlopen) so that single-GPU users need no NCCL at all and so that a host
@@ -162,7 +162,7 @@ struct bdepth {
     uint32_t S = 1;                       // counter sets in the current run (samples, or 1)
     DevBuf rg_ids, rg_offs, rg_samp;
     DevBuf text[2], text_tiles, text_offs, text_zero, text_samp, present;
-    int coll_pending = 0;                 // several ranks: collectives of the current run this rank has not joined yet (2: the sparse decision and the boundary table; 1: the boundary table) -- a rank that stops with an error joins them with a "failed" mark, so that the others stop too instead of waiting for it
+    int coll_pending = 0;                 // several ranks: collectives of the current run this rank has not joined yet (2: the sparse decision and the boundary table; 1: the boundary table; 3: the all-reduce of the flagstat counters) -- a rank that stops with an error joins them with a "failed" mark, so that the others stop too instead of waiting for it
     bool want_presence = false;           // -a with -q and a positive minimum coverage: mark the positions reads cover (k_presence)
     uint64_t batch_u = 6ull << 30;
     uint64_t chunk_blocks = 13 * 32 * 16;              // BGZF blocks per H2D chunk = per K1 sub-launch = per sub-batch: 6656 blocks = 16 K1 CTAs, ~260 MB compressed
@@ -199,6 +199,8 @@ struct bdepth {
     // ---- BAI builder (bdepth_build_index): device tables of k_index_scan, the runs / exceptions it handed out, the finished index
     struct IndexSet { DevBuf lin, lin_len, lin_base, lin_cap, n_mapped, n_unmapped, carry, ctl, runs, excs; std::vector<uint32_t> base, cap; std::vector<IndexRun> h_runs; std::vector<IndexExc> h_excs; uint64_t n_lin = 0; } ix;
     std::vector<uint8_t> built_bai;
+    // ---- flagstat (bdepth_run_flagstat): the counters of k_flagstat plus one word that marks a failed rank in the all-reduce, and their host copy
+    DevBuf fs; uint64_t fs_host[FS_WORDS + 1] = {};
     // ---- several BAM files (bdepth_add_input; MultiBamReader, multireader.d:218-268): the additional files are whole handles that
     // only hold their input (file, BGZF members, header, index, shard / sparse plan); a run swaps them into this handle one after
     // the other and accumulates into the same counters -- per-position counters and per-segment sums are additive over reads,
@@ -456,6 +458,14 @@ void abort_collectives(bdepth* h) {
     const int p = h->coll_pending; h->coll_pending = 0;
     if (!p || h->world <= 1 || !h->comm) return;
     NcclApi& N = nccl(); cudaStream_t sm = h->s_main;
+    if (p == 3) {      // flagstat: the counters' all-reduce, with this rank's "failed" word set
+        uint64_t mark[FS_WORDS + 1] = {}; mark[FS_WORDS] = 1;
+        if (h->fs.ensure(sizeof mark) != cudaSuccess) return;
+        cudaMemcpyAsync(h->fs.p, mark, sizeof mark, cudaMemcpyHostToDevice, sm);
+        N.AllReduce(h->fs.p, h->fs.p, FS_WORDS + 1, NCCL_UINT64, NCCL_SUM, h->comm, sm);
+        cudaStreamSynchronize(sm);
+        return;
+    }
     if (p == 2) {
         uint32_t flag = SPARSE_PEER_FAILED;
         if (h->misc.ensure(16) != cudaSuccess) return;
@@ -638,7 +648,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     bdepth_stats& st = h->st; uint32_t launches0 = 0;
     st = bdepth_stats{}; st.gpu_launches = launches0;
     const bool sparse = mode == RUN_FULL && plan_sparse(h);
-    h->coll_pending = (mode == RUN_FULL && h->world > 1 && h->comm) ? (sparse ? 2 : 1) : 0;
+    h->coll_pending = (mode == RUN_FULL && h->world > 1 && h->comm) ? (sparse ? 2 : 1) : (mode == RUN_FLAGSTAT && h->world > 1 && h->comm) ? 3 : 0;
     if (!sparse) { rc = prepare_shard(h); if (rc) return rc; }      // the plain path needs the whole file's member table (a lazily opened handle frames it now)
     // -m pairs reads of one name wherever they sit in the shard.  A batch is scanned as a whole (no sub-batches), and every
     // batch after the first re-reads the end of the previous one as "ghost" records -- from the earliest record that can
@@ -703,7 +713,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     }
     CK(h->scan_stats.ensure(sizeof(ScanStats)));
     const FilterProg* d_fprog = nullptr;
-    if (h->has_fprog) { CK(h->fprog_d.ensure(sizeof(FilterProg))); CK(cudaMemcpyAsync(h->fprog_d.p, &h->fprog, sizeof(FilterProg), cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm)); d_fprog = h->fprog_d.as<FilterProg>(); }
+    if (h->has_fprog && mode != RUN_FLAGSTAT) { CK(h->fprog_d.ensure(sizeof(FilterProg))); CK(cudaMemcpyAsync(h->fprog_d.p, &h->fprog, sizeof(FilterProg), cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm)); d_fprog = h->fprog_d.as<FilterProg>(); }
     RgTable rgt{nullptr, nullptr, nullptr, 0};
     if (mode == RUN_FULL && (h->S > 1 || (fix && h->hdr.sample_names.size() > 1))) {      // @RG ID -> sample table for the per-read RG lookup (depth.d:240-250); mates pair within a sample
         std::vector<uint8_t> ids; std::vector<uint32_t> offs; std::vector<uint8_t> samp;
@@ -750,6 +760,8 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         IndexCtl c0{0, 0, 0, ~0ull, ~0ull, 0, ~0ull, 0};
         CK(cudaMemcpyAsync(X.ctl.p, &c0, sizeof c0, cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm));
     }
+    float ms_census = 0;
+    if (mode == RUN_FLAGSTAT) { CK(h->fs.ensure((FS_WORDS + 1) * 8)); CK(cudaMemsetAsync(h->fs.p, 0, (FS_WORDS + 1) * 8, sm)); }
     CK(cudaEventRecord(h->ev[10], sm));
     size_t b = blk_lo;
     if (ro) { ro->inflate_len = 0; ro->scan_n = 0; }
@@ -885,7 +897,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
                 CK(cudaEventRecord(h->k1_ev[j], ks));
                 // Sub-batches: a lane needs ~60 ms for its block however empty the GPU is, so the scan / coverage /
                 // delivery of the blocks that arrived first runs while the later chunks are still being inflated.
-                if ((mode == RUN_FULL || mode == RUN_INDEX) && !fix) subs.push_back(Sub{c0, c1, (int)j, (int)j}); else { if (subs.empty()) subs.push_back(Sub{b, b1, 0, (int)j}); subs[0].ev_hi = (int)j; }
+                if ((mode == RUN_FULL || mode == RUN_INDEX || mode == RUN_FLAGSTAT) && !fix) subs.push_back(Sub{c0, c1, (int)j, (int)j}); else { if (subs.empty()) subs.push_back(Sub{b, b1, 0, (int)j}); subs[0].ev_hi = (int)j; }
                 c0 = c1;
             }
         }
@@ -1026,7 +1038,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         const int64_t own_hi = (fix && h->world > 1 && h->limit_abs_u < h->total_u) ? (int64_t)h->limit_abs_u - (int64_t)batch_u0 : INT64_MAX;
         const int64_t zone_below = (!fix && !sparse && h->world > 1) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;       // records of the previous ranks' zone
         UP(h->scan_stats.p, &zs, sizeof zs);
-        if ((mode == RUN_SCAN_ONLY || mode == RUN_INDEX) && !h->ref_has.p) { CK(h->ref_has.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has.p, 0, (nref / 32 + 2) * 4, sm)); }
+        if ((mode == RUN_SCAN_ONLY || mode == RUN_INDEX || mode == RUN_FLAGSTAT) && !h->ref_has.p) { CK(h->ref_has.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has.p, 0, (nref / 32 + 2) * 4, sm)); }
         // runs with -L regions: K2's every-passing-read bits go to a scratch word array, k_ref_seen marks the references of the reads that overlap a region
         uint32_t* has_dst = h->ref_has.as<uint32_t>();
         const uint32_t n_flt_k2 = mode == RUN_FULL ? (uint32_t)h->regions.size() : 0u;
@@ -1047,7 +1059,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         else K2_DECODE(false, false);
 #undef K2_DECODE
         CK(cudaGetLastError()); st.gpu_launches++;
-        if (R && mode != RUN_INDEX && mode != RUN_SCAN_ONLY) {      // quirk 1: CIGARs that begin with N, rewritten to what the reference's cursor makes of them (the index and the raw scan see the file as it is)
+        if (R && mode != RUN_INDEX && mode != RUN_SCAN_ONLY && mode != RUN_FLAGSTAT) {      // quirk 1: CIGARs that begin with N, rewritten to what the reference's cursor makes of them (the index, the raw scan and flagstat see the file as it is)
             // region mode proper (no window slots, no -m, one rank): the statistics of such a read are reproduced (kernels.cuh); otherwise refused
             const bool lead_n_regions = h->seg.on && h->seg.n && !h->seg.has_u && !h->seg.has_min && !fix && h->world == 1;
             LeadNSegs lsg{nullptr, nullptr, nullptr, nullptr, 0u, nullptr, nullptr, 1u, h->minq};
@@ -1207,6 +1219,14 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             { float t = 0; CK(cudaEventElapsedTime(&t, em0, em1)); st.ms_mates += t; }
         }
         CK(cudaEventRecord(e4, sm));
+        // ---- flagstat: the sub-batch's records into the 26 counters (records of the previous rank's zone are that rank's)
+        if (mode == RUN_FLAGSTAT && R) {
+            const int64_t own_from = h->world > 1 ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;
+            CK(cudaEventRecord(h->ev[22], sm));
+            BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_flagstat)(soa, u0, (uint32_t)R, own_from, h->fs.as<unsigned long long>());
+            CK(cudaGetLastError()); st.gpu_launches++;
+            CK(cudaEventRecord(h->ev[23], sm));
+        }
         // Progressive delivery: positions below the start of the sub-batch's last own read are final (the file is coordinate sorted).  Several ranks
         // (plain shards): a rank's own positions begin at its first passing read -- known once such a read has been seen -- and the reads of the
         // previous ranks that reach into them come first in its stream (the zone), so the same holds; where its positions end it learns at the end.
@@ -1222,6 +1242,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             CK(cudaMemcpyAsync(m_u0 - new_carry, u0 + tail, new_carry, cudaMemcpyDeviceToDevice, sm));
         }
         CK(cudaStreamSynchronize(sm));
+        if (mode == RUN_FLAGSTAT && R) { float t; CK(cudaEventElapsedTime(&t, h->ev[22], h->ev[23])); ms_census += t; }
         { float t; if (!h->staged && last_sub) { CK(cudaEventElapsedTime(&t, h->ev[18 + (batch_no & 1)], h->ev[14 + (batch_no & 1)])); ms_h2d += t; } if (last_sub) { CK(cudaEventElapsedTime(&t, e1, e2)); ms_k1 += t; } CK(cudaEventElapsedTime(&t, e2, e3)); ms_k2 += t; CK(cudaEventElapsedTime(&t, e3, e4)); ms_k3 += t; }
         carry_len = (last_batch || fix) ? 0 : new_carry; first_batch = false;
         hs.used = 0;      // synchronised above: the scratch is free again
@@ -1243,6 +1264,15 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         if (sparse_bad) { h->sparse_ok = false; CK(cudaDeviceSynchronize()); return run_pipeline(h, mode, ro, em); }
     }
     st.ms_h2d = ms_h2d; st.ms_inflate = ms_k1; st.ms_scan = ms_k2; st.ms_coverage = ms_k3;
+    if (mode == RUN_FLAGSTAT) {      // several ranks: one all-reduce of the counters; a rank that failed has joined it with its "failed" word set (abort_collectives)
+        if (h->world > 1 && h->comm) { NK(nccl().AllReduce(h->fs.p, h->fs.p, FS_WORDS + 1, NCCL_UINT64, NCCL_SUM, h->comm, sm)); h->coll_pending = 0; }
+        CK(hs.ensure(16384)); hs.used = 0;      // (nothing is in flight: every sub-batch ended synchronised; a run without records has not sized it yet)
+        DOWN(fsp, uint64_t, h->fs.p, (FS_WORDS + 1) * 8);
+        CK(cudaStreamSynchronize(sm));
+        memcpy(h->fs_host, fsp, sizeof h->fs_host);
+        if (h->fs_host[FS_WORDS]) return fail(h, BDEPTH_ERR_NCCL, "another rank of the run stopped with an error (its own message says why): no result");
+        st.ms_reduce = ms_census;
+    }
     st.positions = mode == RUN_FULL ? h->hdr.total_len : 0;
     h->own_lo = 0; h->own_hi = h->hdr.total_len;
     if (mode == RUN_FULL) {
@@ -1950,6 +1980,20 @@ int64_t bdepth_build_index(bdepth_t* h, void* dst, uint64_t cap) {
     }
     if (dst && cap >= h->built_bai.size()) memcpy(dst, h->built_bai.data(), h->built_bai.size());
     return (int64_t)h->built_bai.size();
+}
+
+// ---- flagstat ---------------------------------------------------------------------------------------------------------------------
+// computeFlagStatistics (sambamba/flagstat.d:31-57) over every record of the file (or shard): K1 + K2 as in every run, then k_flagstat per
+// sub-batch.  Nothing in this mode depends on the order of the records, so unsorted input runs as well as sorted input.
+static_assert(sizeof(bdepth_flagstat) == FS_WORDS * sizeof(uint64_t), "bdepth_flagstat holds the 13 categories x 2 QC classes in k_flagstat's order");
+int bdepth_run_flagstat(bdepth_t* h, bdepth_flagstat* out) {
+    if (!h) return BDEPTH_ERR_ARG;
+    if (!out) return fail(h, BDEPTH_ERR_ARG, "null argument");
+    if (!h->extra.empty()) return fail(h, BDEPTH_ERR_ARG, "flagstat reads one BAM file: this handle has several inputs (bdepth_add_input)");
+    int rc = run_pipeline(h, RUN_FLAGSTAT, nullptr); if (rc) return rc;
+    memcpy(out, h->fs_host, sizeof *out);
+    h->st.ms_total_device = h->st.ms_h2d + h->st.ms_inflate + h->st.ms_scan + h->st.ms_coverage + h->st.ms_reduce;
+    return 0;
 }
 
 int bdepth_ref_has_reads(const bdepth_t* h, int ref) {

@@ -5,6 +5,7 @@
 // ("Processing reference #k (name)", "sambamba-depth: <msg>"), same exit codes (0 on usage, 1 on
 // error).  The reference's host language is D, which this image cannot compile (SURVEY F1); the
 // D binding that would replace this file is in sambamba_b200/d/bdepth.d and INTEGRATION.md.
+// Two further subcommands share the engine: `index` (index_main, sambamba/index.d) and `flagstat` (flagstat_main, sambamba/flagstat.d).
 //
 // Not supported through the GPU path yet (rejected with a message, never silently wrong):
 //   -F with back-references / look-around in regular expressions ; several BAM files together with -m ; more than 64 samples without --combined.
@@ -249,11 +250,72 @@ static int index_main(Args& a) {
     return 0;
 }
 
+// percent (flagstat.d:66): to!float(a) / b * 100.0 -- a float quotient, multiplied in double (100.0 is a double literal), returned as float.
+// Printed with "%.2f%%" (:70); Phobos's %.2f of a float is taken to be printf's %.2f of the value widened to double (DESIGN section 8).
+static std::string flagstat_percent(uint64_t a, uint64_t b) {
+    if (b == 0) return "N/A";
+    const float p = (float)((double)((float)a / (float)b) * 100.0);
+    char t[64]; snprintf(t, sizeof t, "%.2f%%", (double)p);
+    return t;
+}
+
+// `sambamba flagstat [-t N] [-p] [-b] input.bam` (flagstat_main, sambamba/flagstat.d:99-150) with the counting on the GPU (bdepth_run_flagstat):
+// -t and -p are accepted and not looked at, -b / --tabular prints CSV.  Every error ends the run as the reference's catch does (:145-148):
+// the message alone on stderr, exit code 1 -- an option std.getopt does not know included.  No input file: usage, exit code 1.
+static int flagstat_main(Args& a) {
+    a.v.erase(a.v.begin() + 1);
+    auto die = [](const std::string& m) { fprintf(stderr, "%s\n", m.c_str()); return 1; };
+    std::vector<std::string> v; std::string cerr_; unsigned long long uv = 0;
+    const int nt = opt_take(a, "nthreads", 't', true, &v);
+    if (nt < 0) return die("Missing value for argument -t.");
+    for (auto& s : v) if (!conv_unsigned(s, 0xFFFFFFFFFFFFFFF0ull, "ulong", uv, cerr_)) return die(cerr_);      // size_t threads
+    opt_take(a, "show-progress", 'p', false, nullptr);
+    const bool tabular = opt_take(a, "tabular", 'b', false, nullptr) > 0;
+    for (size_t i = 1; i < a.v.size(); i++) {
+        if (a.v[i] == "--") { a.v.erase(a.v.begin() + i); break; }
+        if (a.v[i].size() > 1 && a.v[i][0] == '-') return die("Unrecognized option " + a.v[i]);
+    }
+    if (a.v.size() < 2) {
+        fprintf(stderr, "Usage: sambamba-flagstat [options] <input.bam>\n\nOPTIONS: -t, --nthreads=NTHREADS\n            use NTHREADS for decompression\n"
+                        "         -p, --show-progress\n            show progressbar in STDERR\n         -b, --tabular\n            output in csv format\n");
+        return 1;
+    }
+    bdepth_t* h = nullptr;
+    if (bdepth_open(a.v[1].c_str(), 0, &h)) return die(bdepth_last_error(nullptr));
+    bdepth_flagstat fs;
+    if (bdepth_run_flagstat(h, &fs)) { const std::string m = bdepth_last_error(h); bdepth_close(h); return die(m); }
+    bdepth_close(h);
+    auto param = [&](const char* d, const uint64_t* p) {       // writeParam (:59-64)
+        if (tabular) printf("%s,%llu,%llu\n", d, (unsigned long long)p[0], (unsigned long long)p[1]);
+        else printf("%llu + %llu %s\n", (unsigned long long)p[0], (unsigned long long)p[1], d);
+    };
+    auto param_pct = [&](const char* d, const uint64_t* p, const uint64_t* t) {      // writeParamWithPercentage (:73-80)
+        const std::string a0 = flagstat_percent(p[0], t[0]), a1 = flagstat_percent(p[1], t[1]);
+        if (tabular) printf("%s,%llu:%s,%llu:%s\n", d, (unsigned long long)p[0], a0.c_str(), (unsigned long long)p[1], a1.c_str());
+        else printf("%llu + %llu %s (%s:%s)\n", (unsigned long long)p[0], (unsigned long long)p[1], d, a0.c_str(), a1.c_str());
+    };
+    param("in total (QC-passed reads + QC-failed reads)", fs.total);      // :131-143
+    param("secondary", fs.secondary);
+    param("supplementary", fs.supplementary);
+    param("duplicates", fs.duplicates);
+    param_pct("mapped", fs.mapped, fs.total);
+    param("paired in sequencing", fs.paired);
+    param("read1", fs.read1);
+    param("read2", fs.read2);
+    param_pct("properly paired", fs.proper_pair, fs.paired);
+    param("with itself and mate mapped", fs.both_mapped);
+    param_pct("singletons", fs.singletons, fs.paired);
+    param("with mate mapped to a different chr", fs.mate_diff_chr);
+    param("with mate mapped to a different chr (mapQ>=5)", fs.mate_diff_chr_mapq5);
+    return fflush(stdout) == 0 ? 0 : 1;
+}
+
 int main(int argc, char** argv) {
     // accept both `sambamba-depth-b200 base ...` and `sambamba-depth-b200 depth base ...`
     Args a; for (int i = 0; i < argc; i++) a.v.push_back(argv[i]);
     if (a.v.size() > 1 && a.v[1] == "depth") a.v.erase(a.v.begin() + 1);
     if (a.v.size() > 1 && a.v[1] == "index") return index_main(a);
+    if (a.v.size() > 1 && a.v[1] == "flagstat") return flagstat_main(a);
     if (a.v.size() < 3) { usage(); return 0; }
     Ctx c;
     if (a.v[1] == "base") c.mode = 0; else if (a.v[1] == "region") c.mode = 1; else if (a.v[1] == "window") c.mode = 2; else { usage(); return 0; }

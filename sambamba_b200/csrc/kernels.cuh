@@ -1303,6 +1303,43 @@ __global__ void k_ref_seen(RecordSoA soa, uint32_t R, const uint64_t* __restrict
     while (a + 1 < b) { const uint32_t mid = (a + b) >> 1; if (ref_lin0[mid] <= s) a = mid; else b = mid; }
     atomicOr(&ref_has_reads[a >> 5], 1u << (a & 31));
 }
+// ---- sambamba flagstat: computeFlagStatistics (sambamba/flagstat.d:31-57) over one sub-batch, thread per record.  out[2 * c + q]: category c in
+// the order of bdepth_flagstat (include/bdepth.h), q = 1 for QC-failed reads (flag 0x200).  One ballot per category and warp, the warp's leader
+// adds both QC classes into shared memory, and each CTA adds its 26 sums into `out` with one 64-bit atomic per counter.  The flag and MAPQ come
+// from K2's SoA; refID and next_refID are the record's raw fields (the reference compares ref_id != mate_ref_id as written, read.d:86,117).
+// Records below `own_from` (offset of the block_size field, batch-relative) belong to the previous rank's zone and are counted there.
+constexpr int FS_CATEGORIES = 13, FS_WORDS = 2 * FS_CATEGORIES;
+__global__ void __launch_bounds__(256) k_flagstat(RecordSoA soa, const uint8_t* __restrict__ u, uint32_t R, int64_t own_from, unsigned long long* __restrict__ out) {
+    __shared__ uint32_t s_cnt[FS_WORDS];
+    if (threadIdx.x < FS_WORDS) s_cnt[threadIdx.x] = 0;
+    __syncthreads();
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    bool in = r < R;
+    uint32_t flag = 0, mapq = 0; int32_t ref = 0, mate_ref = 0;
+    if (in) {
+        const int64_t o = soa.off[r];                         // refID field
+        in = o - 4 >= own_from;
+        const uint32_t m = soa.meta[r]; flag = m >> 16; mapq = (m >> 8) & 0xFFu;
+        ref = (int32_t)ldu32(u + o); mate_ref = (int32_t)ldu32(u + o + 20);
+    }
+    const bool unmapped = flag & 0x4u, mate_unmapped = flag & 0x8u;
+    const bool secondary = in && (flag & 0x100u);                                   // if (read.is_secondary_alignment)
+    const bool supplementary = in && !secondary && (flag & 0x800u);                 // else if (read.is_supplementary)
+    const bool paired = in && !secondary && !supplementary && (flag & 0x1u);        // else if (read.is_paired)
+    const bool both_mapped = paired && !unmapped && !mate_unmapped;
+    const bool diff_chr = both_mapped && ref != mate_ref;
+    const bool pred[FS_CATEGORIES] = {in, secondary, supplementary, in && (flag & 0x400u), in && !unmapped, paired, paired && (flag & 0x40u), paired && (flag & 0x80u),
+                                      paired && (flag & 0x2u) && !unmapped, both_mapped, paired && mate_unmapped && !unmapped, diff_chr, diff_chr && mapq >= 5u};
+    const uint32_t failed = __ballot_sync(0xFFFFFFFFu, in && (flag & 0x200u));
+#pragma unroll
+    for (int c = 0; c < FS_CATEGORIES; c++) {
+        const uint32_t b = __ballot_sync(0xFFFFFFFFu, pred[c]);
+        if ((threadIdx.x & 31) == 0 && b) { atomicAdd(&s_cnt[2 * c], (uint32_t)__popc(b & ~failed)); atomicAdd(&s_cnt[2 * c + 1], (uint32_t)__popc(b & failed)); }
+    }
+    __syncthreads();
+    if (threadIdx.x < FS_WORDS && s_cnt[threadIdx.x]) atomicAdd(&out[threadIdx.x], (unsigned long long)s_cnt[threadIdx.x]);
+}
+
 __device__ __forceinline__ uint32_t dec_digits(uint32_t v) {
     return v < 10u ? 1u : v < 100u ? 2u : v < 1000u ? 3u : v < 10000u ? 4u : v < 100000u ? 5u : v < 1000000u ? 6u : v < 10000000u ? 7u : v < 100000000u ? 8u : v < 1000000000u ? 9u : 10u;
 }
