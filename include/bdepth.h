@@ -21,6 +21,8 @@
  *     record walk    BioD/bio/std/hts/bam/readrange.d:118-173            bdepth_run_regions(PerBedRegionPrinter, depth.d:879-931)
  *     column sweep   BioD/bio/std/hts/bam/pileup.d:345-424
  *   computeFlagStatistics(bam.reads)     sambamba/flagstat.d:31-57,127   bdepth_run_flagstat (`sambamba flagstat`)
+ *   ReadCounter over view_main's reads   sambamba/view.d:265-379,        bdepth_run_view_count (`sambamba view -c`)
+ *     (filters, -L, regions, '*')        utils/view/alignmentrangeprocessor.d:42-50
  *
  * Conventions: every entry returns 0 on success or a negative bdepth_status; the message is
  * available through bdepth_last_error().  No exception crosses the boundary.  There is no CPU
@@ -251,6 +253,36 @@ typedef struct { uint64_t total[2], secondary[2], supplementary[2], duplicates[2
  * qualities overrun its block_size, a record the reference's release build would count.  Timings: ms_inflate, ms_scan and, for
  * k_flagstat, ms_reduce of bdepth_stats. */
 int bdepth_run_flagstat(bdepth_t* h, bdepth_flagstat* out);
+/* `sambamba view -c` (view.d:265-379): which reads view_main counts.  A read is selected iff every given filter keeps it. */
+enum { BDEPTH_VIEW_ALL = 0, BDEPTH_VIEW_BED = 1, BDEPTH_VIEW_POSITIONAL = 2 };
+typedef struct {
+    uint16_t flag_set, flag_unset;       /* --num-filter=i1/i2 (FlagBitFilter, filtering.d:176-187): (flag & i1) == i1 && (flag & i2) == 0; 0/0 keeps all */
+    const char* query;                   /* -F (createFilterFromQuery, the language bdepth_set_filter_query compiles); NULL or "" keeps all */
+    int subsample;                       /* -s given (a NaN fraction means not given, view.d:286) */
+    uint64_t subsample_threshold;        /* (0x100000000 * fraction).to!ulong (SubsampleFilter, filtering.d:344-347): the caller converts */
+    uint64_t subsampling_seed;           /* --subsampling-seed */
+    int regions_from;                    /* BDEPTH_VIEW_ALL: no regions; BDEPTH_VIEW_BED: -L was given; BDEPTH_VIEW_POSITIONAL: region arguments */
+    const bdepth_region* regions;        /* -L: any order, merged as parseBed merges (bed.d:43-58); positional: one query each, start < end */
+    size_t n_regions;
+    uint32_t n_unmapped;                 /* positional: how many of the region arguments were '*' (unmappedReads, reader.d:370-391) */
+} bdepth_view_opts;
+/* The number `sambamba view -c` prints: ReadCounter (utils/view/alignmentrangeprocessor.d:42-50) over the reads view_main selects, as one call --
+ * options and printing stay with the host.  K1 inflate and the K2 record scan as in every run, then one thread per record (k_view_count).
+ *   - BDEPTH_VIEW_ALL: every record of the file; neither SO:coordinate nor a .bai is needed on one GPU.
+ *   - BDEPTH_VIEW_BED (-L): a read counts once if it reaches a merged region: the first region of its reference whose end lies beyond its position
+ *     has start < pos + basesCovered (BamReadFilter, randomaccessmanager.d:366-462, and BedFilter, filtering.d:118-160, agree on merged regions):
+ *     a zero-length read counts strictly inside a region, not at its start.  On a coordinate-sorted file the .bai is required and only the
+ *     regions' BAI chunks are staged (the whole file when the index does not describe it); on other input the whole file is scanned, and an
+ *     empty region list is BDEPTH_ERR_ARG (the reference's BedFilter indexes it, filtering.d:128).  An empty list on a sorted file counts 0.
+ *   - BDEPTH_VIEW_POSITIONAL (region arguments): each region is its own query and the results are joined: a read counts once per region with
+ *     start < pos + basesCovered and pos < end; start >= end is BDEPTH_ERR_ARG ("start must be less than end", reference.d:77).  Every record
+ *     with refID -1 counts n_unmapped times -- unmappedReads on a coordinate-sorted file, where they form the tail; with n_unmapped > 0 the whole
+ *     file is scanned.  The .bai is required (BDEPTH_ERR_NOINDEX otherwise).
+ * Reads with a negative position count in no region.  The handle's depth settings (filter, -F query, regions, -m, -q, --combined) are not used and
+ * stay set for later runs.  Works on staged input and on bdepth_open_memory handles; a handle with bdepth_add_input files is BDEPTH_ERR_ARG.
+ * Several ranks: each counts its shard (or its share of the region chunks) and one all-reduce sums the counts; a rank that fails makes every rank
+ * return BDEPTH_ERR_NCCL.  Malformed input is BDEPTH_ERR_FORMAT as in every run.  Timings: ms_inflate, ms_scan and, for k_view_count, ms_reduce. */
+int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* opts, uint64_t* count);
 /* Scan records on the GPU; copy out up to cap rows of the columnar SoA (any pointer may be NULL). */
 int64_t bdepth_scan_to_host(bdepth_t* h, uint64_t cap, int32_t* ref_id, int32_t* pos, uint32_t* span, uint16_t* flag, uint8_t* mapq, uint16_t* n_cigar, uint64_t* rec_off);
 

@@ -58,6 +58,21 @@ class FlagStat(C.Structure):
         return {n: (getattr(self, n)[0], getattr(self, n)[1]) for n in FLAGSTAT_FIELDS}
 
 
+class ViewOpts(C.Structure):
+    _fields_ = [("flag_set", C.c_uint16), ("flag_unset", C.c_uint16), ("query", C.c_char_p), ("subsample", C.c_int), ("subsample_threshold", C.c_uint64),
+                ("subsampling_seed", C.c_uint64), ("regions_from", C.c_int), ("regions", C.POINTER(Region)), ("n_regions", C.c_size_t), ("n_unmapped", C.c_uint32)]
+
+
+def subsample_threshold(frac):
+    """SubsampleFilter's threshold (0x100000000 * frac).to!ulong; ValueError where std.conv throws."""
+    t = 4294967296.0 * frac
+    if not t >= 0:
+        raise ValueError("Conversion negative overflow")
+    if t > 18446744073709551616.0:
+        raise ValueError("Conversion positive overflow")
+    return min(int(t), (1 << 64) - 1)
+
+
 class TextOpts(C.Structure):
     _fields_ = [("min_cov", C.c_double), ("max_cov", C.c_double), ("annotate", C.c_int)]
 
@@ -127,6 +142,7 @@ def load_library():
     L.bdepth_build_index.argtypes = [vp, vp, C.c_uint64]
     L.bdepth_build_index.restype = C.c_int64
     L.bdepth_run_flagstat.argtypes = [vp, C.POINTER(FlagStat)]
+    L.bdepth_run_view_count.argtypes = [vp, C.POINTER(ViewOpts), C.POINTER(C.c_uint64)]
     _lib = L
     return L
 
@@ -137,7 +153,7 @@ EXPORTED_SYMBOLS = [
     "bdepth_n_samples", "bdepth_sample_name", "bdepth_set_filter", "bdepth_set_filter_query", "bdepth_set_min_baseq", "bdepth_set_fix_mates", "bdepth_set_combined", "bdepth_set_regions",
     "bdepth_set_shard", "bdepth_nccl_unique_id", "bdepth_plan_shards", "bdepth_plan_region_chunks", "bdepth_set_tuning", "bdepth_stage", "bdepth_run_resident", "bdepth_run_base", "bdepth_run_base_text",
     "bdepth_run_windows", "bdepth_run_regions", "bdepth_get_stats", "bdepth_ref_has_reads", "bdepth_inflate_to_host", "bdepth_scan_to_host", "bdepth_build_index",
-    "bdepth_run_flagstat",
+    "bdepth_run_flagstat", "bdepth_run_view_count",
 ]
 
 
@@ -390,6 +406,22 @@ class BDepth:
         fs = FlagStat()
         self._ck(self.L.bdepth_run_flagstat(self.h, C.byref(fs)))
         return fs.as_dict()
+
+    def run_view_count(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, n_unmapped=0):
+        """`sambamba view -c`: the number of selected reads.  num_filter = (i1, i2); subsample = fraction (with `seed`); bed = [(ref, beg, end)]
+        as -L; regions = [(ref, beg, end)] positional queries, plus n_unmapped '*' queries."""
+        o = ViewOpts()
+        o.flag_set, o.flag_unset = num_filter
+        o.query = query.encode() if query is not None else None
+        if subsample is not None:
+            o.subsample, o.subsample_threshold, o.subsampling_seed = 1, subsample_threshold(subsample), seed
+        rg = bed if bed is not None else (regions or [])
+        arr = (Region * max(len(rg), 1))(*[Region(*r) for r in rg])
+        o.regions_from = 1 if bed is not None else 2 if (rg or n_unmapped) else 0      # BDEPTH_VIEW_BED / _POSITIONAL / _ALL
+        o.regions, o.n_regions, o.n_unmapped = arr, len(rg), n_unmapped
+        n = C.c_uint64()
+        self._ck(self.L.bdepth_run_view_count(self.h, C.byref(o), C.byref(n)))
+        return n.value
 
     def scan(self, cap):
         cols = dict(ref_id=np.zeros(cap, np.int32), pos=np.zeros(cap, np.int32), span=np.zeros(cap, np.uint32),

@@ -80,7 +80,7 @@ constexpr size_t EMIT_CHUNK = 4ull << 20;     // positions per D2H chunk
 constexpr uint32_t SHARD_EXTRA_BLOCKS = 8;
 constexpr uint32_t MATE_ZONE_BLOCKS = 64;       // -m on several ranks: blocks read behind the shard so that pairs cut by the boundary are seen whole
 
-enum RunMode { RUN_FULL = 0, RUN_INFLATE_ONLY = 1, RUN_SCAN_ONLY = 2, RUN_INDEX = 3, RUN_FLAGSTAT = 4 };
+enum RunMode { RUN_FULL = 0, RUN_INFLATE_ONLY = 1, RUN_SCAN_ONLY = 2, RUN_INDEX = 3, RUN_FLAGSTAT = 4, RUN_VIEW_COUNT = 5 };
 constexpr int RC_RETRY_WINDOW = 1;      // internal: a read lies outside the counter window a multi-input run was given
 
 // ---- NCCL, bound at run time (dlopen) so that single-GPU users need no NCCL at all and so that a host
@@ -162,7 +162,7 @@ struct bdepth {
     uint32_t S = 1;                       // counter sets in the current run (samples, or 1)
     DevBuf rg_ids, rg_offs, rg_samp;
     DevBuf text[2], text_tiles, text_offs, text_zero, text_samp, present;
-    int coll_pending = 0;                 // several ranks: collectives of the current run this rank has not joined yet (2: the sparse decision and the boundary table; 1: the boundary table; 3: the all-reduce of the flagstat counters) -- a rank that stops with an error joins them with a "failed" mark, so that the others stop too instead of waiting for it
+    int coll_pending = 0;                 // several ranks: collectives of the current run this rank has not joined yet (2: the sparse decision and the boundary table; 1: the boundary table; 3: the all-reduce of the flagstat counters; 4: that of the view count) -- a rank that stops with an error joins them with a "failed" mark, so that the others stop too instead of waiting for it
     bool want_presence = false;           // -a with -q and a positive minimum coverage: mark the positions reads cover (k_presence)
     uint64_t batch_u = 6ull << 30;
     uint64_t chunk_blocks = 13 * 32 * 16;              // BGZF blocks per H2D chunk = per K1 sub-launch = per sub-batch: 6656 blocks = 16 K1 CTAs, ~260 MB compressed
@@ -201,6 +201,8 @@ struct bdepth {
     std::vector<uint8_t> built_bai;
     // ---- flagstat (bdepth_run_flagstat): the counters of k_flagstat plus one word that marks a failed rank in the all-reduce, and their host copy
     DevBuf fs; uint64_t fs_host[FS_WORDS + 1] = {};
+    // ---- view -c (bdepth_run_view_count): the selection of the current run, its device tables, the count plus a "failed rank" word and their host copy
+    ViewSel vsel{}; DevBuf vc, vc_reg, vc_prog; uint64_t vc_host[2] = {};
     // ---- several BAM files (bdepth_add_input; MultiBamReader, multireader.d:218-268): the additional files are whole handles that
     // only hold their input (file, BGZF members, header, index, shard / sparse plan); a run swaps them into this handle one after
     // the other and accumulates into the same counters -- per-position counters and per-segment sums are additive over reads,
@@ -458,11 +460,12 @@ void abort_collectives(bdepth* h) {
     const int p = h->coll_pending; h->coll_pending = 0;
     if (!p || h->world <= 1 || !h->comm) return;
     NcclApi& N = nccl(); cudaStream_t sm = h->s_main;
-    if (p == 3) {      // flagstat: the counters' all-reduce, with this rank's "failed" word set
-        uint64_t mark[FS_WORDS + 1] = {}; mark[FS_WORDS] = 1;
-        if (h->fs.ensure(sizeof mark) != cudaSuccess) return;
-        cudaMemcpyAsync(h->fs.p, mark, sizeof mark, cudaMemcpyHostToDevice, sm);
-        N.AllReduce(h->fs.p, h->fs.p, FS_WORDS + 1, NCCL_UINT64, NCCL_SUM, h->comm, sm);
+    if (p == 3 || p == 4) {      // flagstat / view -c: the counters' all-reduce, with this rank's "failed" word set
+        uint64_t mark[FS_WORDS + 1] = {}; const size_t nw = p == 3 ? FS_WORDS + 1 : 2; mark[nw - 1] = 1;
+        DevBuf& d = p == 3 ? h->fs : h->vc;
+        if (d.ensure(nw * 8) != cudaSuccess) return;
+        cudaMemcpyAsync(d.p, mark, nw * 8, cudaMemcpyHostToDevice, sm);
+        N.AllReduce(d.p, d.p, nw, NCCL_UINT64, NCCL_SUM, h->comm, sm);
         cudaStreamSynchronize(sm);
         return;
     }
@@ -647,8 +650,8 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     auto t_host0 = std::chrono::steady_clock::now();
     bdepth_stats& st = h->st; uint32_t launches0 = 0;
     st = bdepth_stats{}; st.gpu_launches = launches0;
-    const bool sparse = mode == RUN_FULL && plan_sparse(h);
-    h->coll_pending = (mode == RUN_FULL && h->world > 1 && h->comm) ? (sparse ? 2 : 1) : (mode == RUN_FLAGSTAT && h->world > 1 && h->comm) ? 3 : 0;
+    const bool sparse = (mode == RUN_FULL || mode == RUN_VIEW_COUNT) && plan_sparse(h);      // (view -c: bdepth_run_view_count has put its own regions there)
+    h->coll_pending = (mode == RUN_FULL && h->world > 1 && h->comm) ? (sparse ? 2 : 1) : (mode == RUN_FLAGSTAT && h->world > 1 && h->comm) ? 3 : (mode == RUN_VIEW_COUNT && h->world > 1 && h->comm) ? (sparse ? 2 : 4) : 0;
     if (!sparse) { rc = prepare_shard(h); if (rc) return rc; }      // the plain path needs the whole file's member table (a lazily opened handle frames it now)
     // -m pairs reads of one name wherever they sit in the shard.  A batch is scanned as a whole (no sub-batches), and every
     // batch after the first re-reads the end of the previous one as "ghost" records -- from the earliest record that can
@@ -713,7 +716,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     }
     CK(h->scan_stats.ensure(sizeof(ScanStats)));
     const FilterProg* d_fprog = nullptr;
-    if (h->has_fprog && mode != RUN_FLAGSTAT) { CK(h->fprog_d.ensure(sizeof(FilterProg))); CK(cudaMemcpyAsync(h->fprog_d.p, &h->fprog, sizeof(FilterProg), cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm)); d_fprog = h->fprog_d.as<FilterProg>(); }
+    if (h->has_fprog && mode != RUN_FLAGSTAT && mode != RUN_VIEW_COUNT) { CK(h->fprog_d.ensure(sizeof(FilterProg))); CK(cudaMemcpyAsync(h->fprog_d.p, &h->fprog, sizeof(FilterProg), cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm)); d_fprog = h->fprog_d.as<FilterProg>(); }
     RgTable rgt{nullptr, nullptr, nullptr, 0};
     if (mode == RUN_FULL && (h->S > 1 || (fix && h->hdr.sample_names.size() > 1))) {      // @RG ID -> sample table for the per-read RG lookup (depth.d:240-250); mates pair within a sample
         std::vector<uint8_t> ids; std::vector<uint32_t> offs; std::vector<uint8_t> samp;
@@ -762,6 +765,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     }
     float ms_census = 0;
     if (mode == RUN_FLAGSTAT) { CK(h->fs.ensure((FS_WORDS + 1) * 8)); CK(cudaMemsetAsync(h->fs.p, 0, (FS_WORDS + 1) * 8, sm)); }
+    if (mode == RUN_VIEW_COUNT) { CK(h->vc.ensure(16)); CK(cudaMemsetAsync(h->vc.p, 0, 16, sm)); }
     CK(cudaEventRecord(h->ev[10], sm));
     size_t b = blk_lo;
     if (ro) { ro->inflate_len = 0; ro->scan_n = 0; }
@@ -897,7 +901,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
                 CK(cudaEventRecord(h->k1_ev[j], ks));
                 // Sub-batches: a lane needs ~60 ms for its block however empty the GPU is, so the scan / coverage /
                 // delivery of the blocks that arrived first runs while the later chunks are still being inflated.
-                if ((mode == RUN_FULL || mode == RUN_INDEX || mode == RUN_FLAGSTAT) && !fix) subs.push_back(Sub{c0, c1, (int)j, (int)j}); else { if (subs.empty()) subs.push_back(Sub{b, b1, 0, (int)j}); subs[0].ev_hi = (int)j; }
+                if ((mode == RUN_FULL || mode == RUN_INDEX || mode == RUN_FLAGSTAT || mode == RUN_VIEW_COUNT) && !fix) subs.push_back(Sub{c0, c1, (int)j, (int)j}); else { if (subs.empty()) subs.push_back(Sub{b, b1, 0, (int)j}); subs[0].ev_hi = (int)j; }
                 c0 = c1;
             }
         }
@@ -1038,7 +1042,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         const int64_t own_hi = (fix && h->world > 1 && h->limit_abs_u < h->total_u) ? (int64_t)h->limit_abs_u - (int64_t)batch_u0 : INT64_MAX;
         const int64_t zone_below = (!fix && !sparse && h->world > 1) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;       // records of the previous ranks' zone
         UP(h->scan_stats.p, &zs, sizeof zs);
-        if ((mode == RUN_SCAN_ONLY || mode == RUN_INDEX || mode == RUN_FLAGSTAT) && !h->ref_has.p) { CK(h->ref_has.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has.p, 0, (nref / 32 + 2) * 4, sm)); }
+        if ((mode == RUN_SCAN_ONLY || mode == RUN_INDEX || mode == RUN_FLAGSTAT || mode == RUN_VIEW_COUNT) && !h->ref_has.p) { CK(h->ref_has.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has.p, 0, (nref / 32 + 2) * 4, sm)); }
         // runs with -L regions: K2's every-passing-read bits go to a scratch word array, k_ref_seen marks the references of the reads that overlap a region
         uint32_t* has_dst = h->ref_has.as<uint32_t>();
         const uint32_t n_flt_k2 = mode == RUN_FULL ? (uint32_t)h->regions.size() : 0u;
@@ -1059,7 +1063,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         else K2_DECODE(false, false);
 #undef K2_DECODE
         CK(cudaGetLastError()); st.gpu_launches++;
-        if (R && mode != RUN_INDEX && mode != RUN_SCAN_ONLY && mode != RUN_FLAGSTAT) {      // quirk 1: CIGARs that begin with N, rewritten to what the reference's cursor makes of them (the index, the raw scan and flagstat see the file as it is)
+        if (R && mode != RUN_INDEX && mode != RUN_SCAN_ONLY && mode != RUN_FLAGSTAT && mode != RUN_VIEW_COUNT) {      // quirk 1: CIGARs that begin with N, rewritten to what the reference's cursor makes of them (the index, the raw scan, flagstat and view -c see the file as it is)
             // region mode proper (no window slots, no -m, one rank): the statistics of such a read are reproduced (kernels.cuh); otherwise refused
             const bool lead_n_regions = h->seg.on && h->seg.n && !h->seg.has_u && !h->seg.has_min && !fix && h->world == 1;
             LeadNSegs lsg{nullptr, nullptr, nullptr, nullptr, 0u, nullptr, nullptr, 1u, h->minq};
@@ -1227,6 +1231,14 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             CK(cudaGetLastError()); st.gpu_launches++;
             CK(cudaEventRecord(h->ev[23], sm));
         }
+        // ---- view -c: the sub-batch's selected records into the count (a sparse run on several ranks has no zone: each rank reads its own chunks)
+        if (mode == RUN_VIEW_COUNT && R) {
+            const int64_t own_from = (h->world > 1 && !sparse) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;
+            CK(cudaEventRecord(h->ev[22], sm));
+            BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_view_count)(soa, u0, (uint32_t)R, own_from, h->vsel, h->vc.as<unsigned long long>());
+            CK(cudaGetLastError()); st.gpu_launches++;
+            CK(cudaEventRecord(h->ev[23], sm));
+        }
         // Progressive delivery: positions below the start of the sub-batch's last own read are final (the file is coordinate sorted).  Several ranks
         // (plain shards): a rank's own positions begin at its first passing read -- known once such a read has been seen -- and the reads of the
         // previous ranks that reach into them come first in its stream (the zone), so the same holds; where its positions end it learns at the end.
@@ -1242,7 +1254,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             CK(cudaMemcpyAsync(m_u0 - new_carry, u0 + tail, new_carry, cudaMemcpyDeviceToDevice, sm));
         }
         CK(cudaStreamSynchronize(sm));
-        if (mode == RUN_FLAGSTAT && R) { float t; CK(cudaEventElapsedTime(&t, h->ev[22], h->ev[23])); ms_census += t; }
+        if ((mode == RUN_FLAGSTAT || mode == RUN_VIEW_COUNT) && R) { float t; CK(cudaEventElapsedTime(&t, h->ev[22], h->ev[23])); ms_census += t; }
         { float t; if (!h->staged && last_sub) { CK(cudaEventElapsedTime(&t, h->ev[18 + (batch_no & 1)], h->ev[14 + (batch_no & 1)])); ms_h2d += t; } if (last_sub) { CK(cudaEventElapsedTime(&t, e1, e2)); ms_k1 += t; } CK(cudaEventElapsedTime(&t, e2, e3)); ms_k2 += t; CK(cudaEventElapsedTime(&t, e3, e4)); ms_k3 += t; }
         carry_len = (last_batch || fix) ? 0 : new_carry; first_batch = false;
         hs.used = 0;      // synchronised above: the scratch is free again
@@ -1256,7 +1268,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             uint32_t flag = sparse_bad ? 1u : 0u;
             CK(cudaMemcpyAsync(h->misc.p, &flag, 4, cudaMemcpyHostToDevice, sm));
             NK(nccl().AllReduce(h->misc.p, h->misc.p, 1, NCCL_UINT32, NCCL_SUM, h->comm, sm));
-            h->coll_pending = 1;
+            h->coll_pending = mode == RUN_VIEW_COUNT ? 4 : 1;
             CK(cudaMemcpyAsync(&flag, h->misc.p, 4, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
             if (flag >= SPARSE_PEER_FAILED) { h->coll_pending = 0; return fail(h, BDEPTH_ERR_NCCL, "another rank of the run stopped with an error (its own message says why): no result"); }
             sparse_bad = flag != 0;
@@ -1271,6 +1283,15 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         CK(cudaStreamSynchronize(sm));
         memcpy(h->fs_host, fsp, sizeof h->fs_host);
         if (h->fs_host[FS_WORDS]) return fail(h, BDEPTH_ERR_NCCL, "another rank of the run stopped with an error (its own message says why): no result");
+        st.ms_reduce = ms_census;
+    }
+    if (mode == RUN_VIEW_COUNT) {      // several ranks: one all-reduce of the count and the "failed" word (abort_collectives), as for flagstat
+        if (h->world > 1 && h->comm) { NK(nccl().AllReduce(h->vc.p, h->vc.p, 2, NCCL_UINT64, NCCL_SUM, h->comm, sm)); h->coll_pending = 0; }
+        CK(hs.ensure(16384)); hs.used = 0;
+        DOWN(vcp, uint64_t, h->vc.p, 16);
+        CK(cudaStreamSynchronize(sm));
+        memcpy(h->vc_host, vcp, sizeof h->vc_host);
+        if (h->vc_host[1]) return fail(h, BDEPTH_ERR_NCCL, "another rank of the run stopped with an error (its own message says why): no result");
         st.ms_reduce = ms_census;
     }
     st.positions = mode == RUN_FULL ? h->hdr.total_len : 0;
@@ -1456,6 +1477,7 @@ void bdepth_close(bdepth_t* h) {
     h->seg.s.release(); h->seg.e.release(); h->seg.pmax.release(); h->seg.id.release(); h->seg.reads.release(); h->seg.minstart.release(); h->seg.bases_reads.release(); h->seg.mbases.release(); h->seg.ustart.release(); h->seg.dscr.release(); h->seg.da.release(); h->seg.dac.release(); h->seg.db.release(); h->seg.dthr.release(); h->seg.dbases.release(); h->seg.dcov.release();
     { auto& X = h->ix; X.lin.release(); X.lin_len.release(); X.lin_base.release(); X.lin_cap.release(); X.n_mapped.release(); X.n_unmapped.release(); X.carry.release(); X.ctl.release(); X.runs.release(); X.excs.release(); }
     h->m_hash.release(); h->m_flag.release(); h->m_flt.release(); h->m_ctl.release(); h->fprog_d.release();
+    h->vc.release(); h->vc_reg.release(); h->vc_prog.release();
     if (h->comm) { nccl().CommDestroy(h->comm); h->comm = nullptr; }
     if (h->pinned) cudaFreeHost(h->pinned);
     h->hs.release();
@@ -1992,6 +2014,84 @@ int bdepth_run_flagstat(bdepth_t* h, bdepth_flagstat* out) {
     if (!h->extra.empty()) return fail(h, BDEPTH_ERR_ARG, "flagstat reads one BAM file: this handle has several inputs (bdepth_add_input)");
     int rc = run_pipeline(h, RUN_FLAGSTAT, nullptr); if (rc) return rc;
     memcpy(out, h->fs_host, sizeof *out);
+    h->st.ms_total_device = h->st.ms_h2d + h->st.ms_inflate + h->st.ms_scan + h->st.ms_coverage + h->st.ms_reduce;
+    return 0;
+}
+
+// ---- view -c ----------------------------------------------------------------------------------------------------------------------
+// ReadCounter over view_main's selection (sambamba/view.d:265-368): K1 + K2 as in every run, then k_view_count per sub-batch.  Regions on a
+// coordinate-sorted file with a usable index stage only their BAI chunks (plan_sparse, with the view's regions in place of the handle's for the
+// duration of the run); otherwise every record of the file is scanned.  The handle's depth settings are not used and stay as they were.
+int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* o, uint64_t* count) {
+    if (!h) return BDEPTH_ERR_ARG;
+    if (!o || !count || (o->n_regions && !o->regions)) return fail(h, BDEPTH_ERR_ARG, "null argument");
+    if (o->regions_from < BDEPTH_VIEW_ALL || o->regions_from > BDEPTH_VIEW_POSITIONAL) return fail(h, BDEPTH_ERR_ARG, "regions_from: %d", o->regions_from);
+    const bool positional = o->regions_from == BDEPTH_VIEW_POSITIONAL;
+    if (!h->extra.empty()) return fail(h, BDEPTH_ERR_ARG, "view reads one BAM file: this handle has several inputs (bdepth_add_input)");
+    const size_t nref = h->hdr.ref_len.size();
+    ViewSel vs{}; vs.flag_set = o->flag_set; vs.flag_unset = o->flag_unset;
+    vs.subsample = o->subsample ? 1u : 0u; vs.threshold = o->subsample_threshold; vs.seed = o->subsampling_seed;
+    FilterProg prog; bool has_prog = false;
+    if (o->query && *o->query) {      // "" is the NullFilter (filtering.d:41-42)
+        FilterCompiler fc(h->hdr.ref_names);
+        const std::string e = fc.compile(o->query, prog);
+        if (!e.empty()) return fail(h, BDEPTH_ERR_ARG, "%s", e.c_str());
+        has_prog = true;
+    }
+    std::vector<bdepth_region> rg;
+    for (size_t i = 0; i < o->n_regions; i++) {
+        const bdepth_region& g = o->regions[i];
+        if (g.ref_id >= nref) return fail(h, BDEPTH_ERR_ARG, "region #%zu: reference %u out of range", i, g.ref_id);
+        if (g.start >= g.end) { if (positional) return fail(h, BDEPTH_ERR_ARG, "start must be less than end"); continue; }      // opSlice, reference.d:77; parseBed keeps beg < end only
+        rg.push_back(g);
+    }
+    const bool sorted = h->hdr.so_coordinate;
+    if (positional) vs.region_mode = (rg.empty() && !o->n_unmapped) ? VIEW_ALL : VIEW_POSITIONAL;
+    else vs.region_mode = o->regions_from == BDEPTH_VIEW_BED ? VIEW_MERGED : VIEW_ALL;
+    vs.n_star = positional ? o->n_unmapped : 0;
+    if (vs.region_mode == VIEW_MERGED && rg.empty()) {
+        if (!sorted) return fail(h, BDEPTH_ERR_ARG, "-L on a file that is not coordinate-sorted names no region of the file's references: the reference's BedFilter indexes an empty region list (filtering.d:128)");
+        *count = 0; h->st = bdepth_stats{}; return 0;                                     // getReadsOverlapping([]): an empty stream
+    }
+    if (vs.region_mode == VIEW_POSITIONAL || (vs.region_mode == VIEW_MERGED && sorted))
+        if (!h->has_index) return fail(h, BDEPTH_ERR_NOINDEX, "BAM index file (.bai) must be provided");      // randomaccessmanager.d:197-202
+    // per-reference slices: starts and ends each sorted (BED: merged as parseBed merges, touching regions included, bed.d:43-58)
+    std::vector<bdepth_region> plan;
+    if (vs.region_mode != VIEW_ALL) {
+        std::vector<uint32_t> off(nref + 1, 0), S, E;
+        if (vs.region_mode == VIEW_MERGED) {
+            std::sort(rg.begin(), rg.end(), [](const bdepth_region& a, const bdepth_region& b) { return a.ref_id != b.ref_id ? a.ref_id < b.ref_id : a.start < b.start; });
+            size_t m = 0;
+            for (size_t i = 0; i < rg.size(); i++) { if (m && rg[m - 1].ref_id == rg[i].ref_id && rg[m - 1].end >= rg[i].start) rg[m - 1].end = std::max(rg[m - 1].end, rg[i].end); else rg[m++] = rg[i]; }
+            rg.resize(m);
+            for (auto& g : rg) { S.push_back(g.start); E.push_back(g.end); off[g.ref_id + 1]++; }
+        } else {
+            std::vector<std::vector<uint32_t>> s(nref), e(nref);
+            for (auto& g : rg) { s[g.ref_id].push_back(g.start); e[g.ref_id].push_back(g.end); off[g.ref_id + 1]++; }
+            for (size_t r = 0; r < nref; r++) { std::sort(s[r].begin(), s[r].end()); std::sort(e[r].begin(), e[r].end()); S.insert(S.end(), s[r].begin(), s[r].end()); E.insert(E.end(), e[r].begin(), e[r].end()); }
+        }
+        for (size_t r = 0; r < nref; r++) off[r + 1] += off[r];
+        int rc = init_device(h); if (rc) return rc;
+        const size_t n = S.size();
+        CK(h->vc_reg.ensure((nref + 1 + 2 * n + 1) * 4));
+        uint32_t* d = h->vc_reg.as<uint32_t>();
+        CK(cudaMemcpy(d, off.data(), (nref + 1) * 4, cudaMemcpyHostToDevice));
+        if (n) { CK(cudaMemcpy(d + nref + 1, S.data(), n * 4, cudaMemcpyHostToDevice)); CK(cudaMemcpy(d + nref + 1 + n, E.data(), n * 4, cudaMemcpyHostToDevice)); }
+        vs.n_reg_refs = (uint32_t)nref; vs.reg_off = d; vs.reg_s = d + nref + 1; vs.reg_e = d + nref + 1 + n;
+        // what to stage: the regions' BAI chunks on a sorted file; the whole file for '*' (the unplaced tail) and for unsorted input
+        if (sorted && !vs.n_star) normalize_regions(h, rg.data(), rg.size(), plan);
+    }
+    if (has_prog) {
+        int rc = init_device(h); if (rc) return rc;
+        CK(h->vc_prog.ensure(sizeof(FilterProg))); CK(cudaMemcpy(h->vc_prog.p, &prog, sizeof(FilterProg), cudaMemcpyHostToDevice));
+        vs.fprog = h->vc_prog.as<FilterProg>();
+    }
+    h->vsel = vs;
+    std::swap(h->regions, plan);
+    const int rc = run_pipeline(h, RUN_VIEW_COUNT, nullptr);
+    std::swap(h->regions, plan);
+    if (rc) return rc;
+    *count = h->vc_host[0];
     h->st.ms_total_device = h->st.ms_h2d + h->st.ms_inflate + h->st.ms_scan + h->st.ms_coverage + h->st.ms_reduce;
     return 0;
 }

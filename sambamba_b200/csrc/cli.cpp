@@ -5,15 +5,18 @@
 // ("Processing reference #k (name)", "sambamba-depth: <msg>"), same exit codes (0 on usage, 1 on
 // error).  The reference's host language is D, which this image cannot compile (SURVEY F1); the
 // D binding that would replace this file is in sambamba_b200/d/bdepth.d and INTEGRATION.md.
-// Two further subcommands share the engine: `index` (index_main, sambamba/index.d) and `flagstat` (flagstat_main, sambamba/flagstat.d).
+// Three further subcommands share the engine: `index` (index_main, sambamba/index.d), `flagstat` (flagstat_main, sambamba/flagstat.d) and
+// `view -c` (view_main, sambamba/view.d; the count only).
 //
 // Not supported through the GPU path yet (rejected with a message, never silently wrong):
 //   -F with back-references / look-around in regular expressions ; several BAM files together with -m ; more than 64 samples without --combined.
+#include <errno.h>
 #include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <time.h>
 #include <algorithm>
 #include <string>
 #include <vector>
@@ -310,12 +313,127 @@ static int flagstat_main(Args& a) {
     return fflush(stdout) == 0 ? 0 : 1;
 }
 
+// `sambamba view -c [options] input.bam [region ...]` (view_main / sambambaMain, sambamba/view.d:149-379) with the counting on the GPU
+// (bdepth_run_view_count).  Only the count is offered: without -c, and with -v (validation), -S (SAM input) or -T, the run ends with a
+// "not supported" message instead of printing records.  -h, -f, -l, -p, -t and -I are accepted and change nothing of the count; -c -H prints
+// nothing.  -o FILE is created or truncated as the reference opens it (w+), while the count goes to stdout.  Every error: "sambamba-view: <msg>",
+// exit code 1.  No input file: usage, exit code 0.
+static int view_main(Args& a) {
+    a.v.erase(a.v.begin() + 1);
+    auto die = [](const std::string& m) { fprintf(stderr, "sambamba-view: %s\n", m.c_str()); return 1; };
+    std::string cerr_; unsigned long long uv = 0;
+    std::string query, numfilter, format = "sam", bed_fn, out_fn, ref_fn; bool has_query = false, has_numfilter = false, has_bed = false, has_out = false, has_ref_fn = false;
+    double frac = NAN; unsigned long long seed = 0; bool has_seed = false;
+    struct StrOpt { const char* lng; char sht; std::string* dst; bool* given; };
+    const StrOpt sopts[] = {{"filter", 'F', &query, &has_query}, {"num-filter", 0, &numfilter, &has_numfilter}, {"format", 'f', &format, nullptr},
+                            {"regions", 'L', &bed_fn, &has_bed}, {"output-filename", 'o', &out_fn, &has_out}, {"ref-filename", 'T', &ref_fn, &has_ref_fn}};
+    std::vector<std::string> v;
+    for (const StrOpt& so : sopts) {
+        v.clear();
+        const int n = opt_take(a, so.lng, so.sht, true, &v);
+        if (n < 0) return die(std::string("Missing value for argument ") + (so.sht ? std::string("-") + so.sht : std::string("--") + so.lng) + ".");
+        if (n > 0) { *so.dst = v.back(); if (so.given) *so.given = true; }
+    }
+    opt_take(a, "with-header", 'h', false, nullptr);
+    const bool header_only = opt_take(a, "header", 'H', false, nullptr) > 0;
+    opt_take(a, "reference-info", 'I', false, nullptr);                     // with -c: counts (view.d:243)
+    const bool count_only = opt_take(a, "count", 'c', false, nullptr) > 0, valid = opt_take(a, "valid", 'v', false, nullptr) > 0, sam_in = opt_take(a, "sam-input", 'S', false, nullptr) > 0;
+    opt_take(a, "show-progress", 'p', false, nullptr);
+    struct NumOpt { const char* lng; char sht; };
+    for (const NumOpt& no : {NumOpt{"compression-level", 'l'}, NumOpt{"nthreads", 't'}, NumOpt{"subsample", 's'}, NumOpt{"subsampling-seed", 0}}) {
+        v.clear();
+        const int n = opt_take(a, no.lng, no.sht, true, &v);
+        if (n < 0) return die(std::string("Missing value for argument ") + (no.sht ? std::string("-") + no.sht : std::string("--") + no.lng) + ".");
+        for (const std::string& s : v) {
+            if (no.sht == 'l') { const bool neg = !s.empty() && s[0] == '-'; if (!conv_unsigned(neg ? s.substr(1) : s, neg ? 0x80000000ull : 0x7FFFFFFFull, "int", uv, cerr_)) return die(cerr_); }
+            else if (no.sht == 't') { if (!conv_unsigned(s, 0xFFFFFFFFull, "uint", uv, cerr_)) return die(cerr_); }
+            else if (no.sht == 's') { if (!conv_double(s, frac, cerr_)) return die(cerr_); }
+            else { if (!conv_unsigned(s, 0xFFFFFFFFFFFFFFF0ull, "ulong", uv, cerr_)) return die(cerr_); seed = uv; has_seed = true; }
+        }
+    }
+    for (size_t i = 1; i < a.v.size(); i++) {
+        if (a.v[i] == "--") { a.v.erase(a.v.begin() + i); break; }
+        if (a.v[i].size() > 1 && a.v[i][0] == '-') return die("Unrecognized option " + a.v[i]);
+    }
+    if (a.v.size() < 2) {
+        fprintf(stderr, "Usage: sambamba-view -c [options] <input.bam> [region1 [...]]\n\n"
+                        "Counts the reads `sambamba view` would output, on the GPU.  Only the count (-c) is supported.\n\n"
+                        "Options: -F, --filter=FILTER   --num-filter=I1/I2   -L, --regions=FILENAME   -c, --count\n"
+                        "         -s, --subsample=FRACTION   --subsampling-seed=SEED   -o, --output-filename=FILE\n"
+                        "         accepted and without effect on the count: -h, -H, -I, -f, -l, -p, -t\n");
+        return 0;
+    }
+    const std::string bam_path = a.v[1];
+    if (has_out && out_fn == bam_path) return die("Specified output filename " + out_fn + " clashes with one of input file names. Exiting.");      // protectFromOverwrite
+    // what this GPU path does not produce: refused before anything is opened
+    if (!count_only) return die("not supported: only the count (-c) is computed on the GPU; record output (SAM, BAM, JSON, the header, -I) is not");
+    if (valid) return die("not supported: -v (skip invalid alignments) is not available with -c on the GPU");
+    if (sam_in) return die("not supported: -S (SAM input); the GPU path reads BAM");
+    if (has_ref_fn) return die("not supported: -T (reference FASTA)");
+    if (format == "unpack") return die("not supported: -f unpack");
+    if (has_out && out_fn != "-") {                    // File(output_filename, "w+") (view.d:204): created or truncated, nothing written to it
+        FILE* f = fopen(out_fn.c_str(), "w+");
+        if (!f) return die("Cannot open file `" + out_fn + "' in mode `w+' (" + strerror(errno) + ")");
+        fclose(f);
+    }
+    bdepth_t* h = nullptr;
+    if (bdepth_open_lazy(bam_path.c_str(), 0, &h)) return die(bdepth_last_error(nullptr));
+    struct Closer { bdepth_t* h; ~Closer() { bdepth_close(h); } } closer{h};
+    if (header_only) return 0;                         // view.d:260-263
+    bdepth_view_opts o{};
+    if (has_numfilter) {                               // view.d:271-277: "i1/i2", either may be empty
+        std::vector<std::string> m; size_t p = 0;
+        for (;;) { size_t q = numfilter.find('/', p); m.push_back(numfilter.substr(p, q == std::string::npos ? std::string::npos : q - p)); if (q == std::string::npos) break; p = q + 1; }
+        if (!m.empty() && !m[0].empty()) { if (!conv_unsigned(m[0], 0xFFFF, "ushort", uv, cerr_)) return die(cerr_); o.flag_set = (uint16_t)uv; }
+        if (m.size() > 1 && !m[1].empty()) { if (!conv_unsigned(m[1], 0xFFFF, "ushort", uv, cerr_)) return die(cerr_); o.flag_unset = (uint16_t)uv; }
+    }
+    o.query = has_query ? query.c_str() : nullptr;
+    if (!isnan(frac)) {                                // SubsampleFilter: (0x100000000UL * frac).to!ulong (filtering.d:344-347)
+        const double t = 4294967296.0 * frac;
+        if (!(t >= 0)) return die("Conversion negative overflow");
+        if (t > 18446744073709551616.0) return die("Conversion positive overflow");
+        o.subsample = 1; o.subsample_threshold = t >= 18446744073709551616.0 ? UINT64_MAX : (uint64_t)t;
+        if (!has_seed) { FILE* r = fopen("/dev/urandom", "rb"); if (!r || fread(&seed, 8, 1, r) != 1) seed = (unsigned long long)time(nullptr); if (r) fclose(r); }      // view.d:160-162: an unpredictable seed
+        o.subsampling_seed = seed;
+    }
+    if (has_bed && a.v.size() > 2) return die("specifying both region and BED filename is disallowed");
+    const int nref = bdepth_n_ref(h);
+    auto find_ref = [&](const std::string& n) { for (int i = 0; i < nref; i++) if (n == bdepth_ref_name(h, i)) return i; return -1; };
+    std::vector<bdepth_region> regs;
+    o.regions_from = has_bed ? BDEPTH_VIEW_BED : BDEPTH_VIEW_POSITIONAL;
+    if (has_bed) {                                     // parseBed (bed.d:128-152): regions on unknown references are left out
+        FILE* f = fopen(bed_fn.c_str(), "rb");
+        if (!f) return die(bed_fn + ": " + strerror(errno));
+        fclose(f);
+        std::vector<BedIv> ivs; std::vector<std::string> lines;
+        if (!bed_read(bed_fn, ivs, lines)) return die("cannot parse BED file " + bed_fn);
+        for (auto& iv : ivs) { const int id = find_ref(iv.chr); if (id >= 0) regs.push_back({(uint32_t)id, (uint32_t)iv.beg, (uint32_t)iv.end}); }
+    } else {
+        for (size_t i = 2; i < a.v.size(); i++) {      // view.d:346-358, in order: the first bad region ends the run
+            if (a.v[i] == "*") { if (!bdepth_has_index(h)) return die("BAM index file (.bai) must be provided"); o.n_unmapped++; continue; }
+            std::string ref; uint32_t beg, end; parse_region_string(a.v[i], ref, beg, end);
+            const int id = find_ref(ref);
+            if (id < 0) return die("Reference with name " + ref + " does not exist");
+            if (end == UINT32_MAX) end = bdepth_ref_length(h, id);
+            if (!(beg < end)) return die("start must be less than end");
+            if (!bdepth_has_index(h)) return die("BAM index file (.bai) must be provided");
+            regs.push_back({(uint32_t)id, beg, end});
+        }
+    }
+    o.regions = regs.data(); o.n_regions = regs.size();
+    uint64_t n = 0;
+    if (bdepth_run_view_count(h, &o, &n)) return die(bdepth_last_error(h));
+    printf("%llu\n", (unsigned long long)n);
+    return fflush(stdout) == 0 ? 0 : 1;
+}
+
 int main(int argc, char** argv) {
     // accept both `sambamba-depth-b200 base ...` and `sambamba-depth-b200 depth base ...`
     Args a; for (int i = 0; i < argc; i++) a.v.push_back(argv[i]);
     if (a.v.size() > 1 && a.v[1] == "depth") a.v.erase(a.v.begin() + 1);
     if (a.v.size() > 1 && a.v[1] == "index") return index_main(a);
     if (a.v.size() > 1 && a.v[1] == "flagstat") return flagstat_main(a);
+    if (a.v.size() > 1 && a.v[1] == "view") return view_main(a);
     if (a.v.size() < 3) { usage(); return 0; }
     Ctx c;
     if (a.v[1] == "base") c.mode = 0; else if (a.v[1] == "region") c.mode = 1; else if (a.v[1] == "window") c.mode = 2; else { usage(); return 0; }

@@ -1340,6 +1340,73 @@ __global__ void __launch_bounds__(256) k_flagstat(RecordSoA soa, const uint8_t* 
     if (threadIdx.x < FS_WORDS && s_cnt[threadIdx.x]) atomicAdd(&out[threadIdx.x], (unsigned long long)s_cnt[threadIdx.x]);
 }
 
+// ---- sambamba view -c: ReadCounter (utils/view/alignmentrangeprocessor.d:42-50) over the reads view_main selects (sambamba/view.d:265-368), one
+// sub-batch, thread per record.  A record adds its multiplicity -- how often the reference's joined stream holds it -- if it passes
+//   * --num-filter (FlagBitFilter, filtering.d:176-187): (flag & flag_set) == flag_set && (flag & flag_unset) == 0;
+//   * -s (SubsampleFilter, :340-371): FNV-1a 64 over the read name, then the 8 little-endian bytes of the seed; kept iff the low 32 bits < threshold;
+//   * -F: the compiled query (filter.cuh).  Not K2's pass bit, which also demands a placed, mapped read with span > 0.
+// Multiplicity, with bc = basesCovered (read.d:255-262: 0 for an unmapped read, else the reference-consuming CIGAR lengths as written):
+//   VIEW_ALL         1.
+//   VIEW_MERGED      -L: 1 iff the first merged region of the read's reference whose end lies beyond pos has start < pos + bc -- BamReadFilter's state
+//                    machine (randomaccessmanager.d:366-462) on a sorted file, and equally BedFilter's interval overlap (filtering.d:118-160) on
+//                    merged regions: a zero-length read counts strictly inside a region, not at its start.
+//   VIEW_POSITIONAL  one bam[ref][beg..end] query per region, joined: #{start < pos + bc} - #{end <= pos} over the reference's sorted starts and
+//                    sorted ends (every region has start < end, so each region with end <= pos also has start < pos + bc); a record with
+//                    refID -1 counts n_star times ('*', unmappedReads, reader.d:370-391).
+// Reads with pos < 0 on a reference count in no region.  Records below `own_from` (offset of the block_size field, batch-relative) belong to the
+// previous rank's zone and are counted there.  Warp sum, one shared word per CTA, one 64-bit atomic per CTA.
+constexpr uint32_t VIEW_ALL = 0, VIEW_MERGED = 1, VIEW_POSITIONAL = 2;
+struct ViewSel {
+    uint32_t flag_set, flag_unset;
+    const FilterProg* fprog;                       // nullptr: no -F
+    uint32_t subsample; unsigned long long threshold, seed;
+    uint32_t region_mode, n_star;
+    uint32_t n_reg_refs;                           // references with a slice: reg_off has n_reg_refs + 1 entries
+    const uint32_t* reg_off; const uint32_t* reg_s; const uint32_t* reg_e;      // regions of reference r: [reg_off[r], reg_off[r + 1]), starts and ends each sorted
+};
+__global__ void __launch_bounds__(256) k_view_count(RecordSoA soa, const uint8_t* __restrict__ u, uint32_t R, int64_t own_from, ViewSel vs, unsigned long long* __restrict__ out) {
+    __shared__ unsigned long long s_sum;
+    if (threadIdx.x == 0) s_sum = 0;
+    __syncthreads();
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long m = 0;
+    if (r < R && soa.off[r] - 4 >= own_from) {
+        const int64_t o = soa.off[r];                          // refID field
+        const uint32_t flag = soa.meta[r] >> 16, ncl = soa.ncl[r], l_name = ncl & 0xFFu, n_cigar = (ncl >> 8) & 0xFFFFu;
+        bool keep = (flag & vs.flag_set) == vs.flag_set && (flag & vs.flag_unset) == 0;
+        if (keep && vs.subsample) {
+            unsigned long long h = 14695981039346656037ull;
+            for (uint32_t i = 0; i + 1 < l_name; i++) { h ^= u[o + 32 + i]; h *= 1099511628211ull; }      // read.name: l_name - 1 bytes, without the NUL
+            for (int i = 0; i < 8; i++) { h ^= (vs.seed >> (8 * i)) & 0xFFu; h *= 1099511628211ull; }
+            keep = (h & 0xFFFFFFFFull) < vs.threshold;
+        }
+        if (keep && vs.fprog) keep = filter_eval_cold(vs.fprog, u + o, ldu32(u + o - 4));
+        if (keep && vs.region_mode == VIEW_ALL) m = 1;
+        else if (keep) {
+            const int32_t ref = (int32_t)ldu32(u + o), pos = (int32_t)ldu32(u + o + 4);
+            if (ref < 0) m = vs.region_mode == VIEW_POSITIONAL ? vs.n_star : 0u;
+            else if ((uint32_t)ref < vs.n_reg_refs && pos >= 0) {
+                uint64_t bc = 0;
+                if (!(flag & 4u)) { const uint8_t* cg = u + o + 32 + l_name; for (uint32_t i = 0; i < n_cigar; i++) { const uint32_t c = ldu32(cg + 4 * i); if (cig_rcons(c & 15)) bc += c >> 4; } }
+                const uint64_t p = (uint32_t)pos, e = p + bc;
+                const uint32_t lo = vs.reg_off[ref], hi = vs.reg_off[ref + 1];
+                uint32_t a = lo, b = hi;                                             // first region with end > p
+                while (a < b) { const uint32_t mid = (a + b) >> 1; if (vs.reg_e[mid] > p) b = mid; else a = mid + 1; }
+                if (vs.region_mode == VIEW_MERGED) m = (a < hi && vs.reg_s[a] < e) ? 1u : 0u;
+                else {
+                    uint32_t c = lo, d = hi;                                         // regions with start < p + bc
+                    while (c < d) { const uint32_t mid = (c + d) >> 1; if (vs.reg_s[mid] < e) c = mid + 1; else d = mid; }
+                    m = (unsigned long long)(c - lo) - (a - lo);
+                }
+            }
+        }
+    }
+    for (int s = 16; s; s >>= 1) m += __shfl_xor_sync(0xFFFFFFFFu, m, s);
+    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&s_sum, m);
+    __syncthreads();
+    if (threadIdx.x == 0 && s_sum) atomicAdd(out, s_sum);
+}
+
 __device__ __forceinline__ uint32_t dec_digits(uint32_t v) {
     return v < 10u ? 1u : v < 100u ? 2u : v < 1000u ? 3u : v < 10000u ? 4u : v < 100000u ? 5u : v < 1000000u ? 6u : v < 10000000u ? 7u : v < 100000000u ? 8u : v < 1000000000u ? 9u : 10u;
 }

@@ -1,0 +1,271 @@
+/* view_count_oracle.c -- CPU restatement of `sambamba view -c` (TEST INFRASTRUCTURE: the checker the GPU count is compared with).
+ *
+ * What is restated (sambamba/view.d:265-379), record by record, without shortcuts:
+ *   - FlagBitFilter (utils/common/filtering.d:176-187) and SubsampleFilter (:340-371, FNV-1a 64 over the name, then the seed's 8 bytes);
+ *   - -L on a file that is not SO:coordinate: BedFilter (:118-160), its interval-tree overlap rule iv.stop > start && iv.start < stop on
+ *     unsigned coordinates (utils/common/intervaltree.d:122-131), checked against every region of the read's reference;
+ *   - -L on a sorted file: getReadsOverlapping (randomaccessmanager.d:316-338) -- regions grouped by reference, each group walked by the
+ *     BamReadFilter state machine (:366-462) over the file's records;
+ *   - positional regions: one BamReadFilter with one region per argument, the streams joined; '*' is unmappedReads (reader.d:370-391): skip to
+ *     the first record with refID -1, then every record to the end of the file.
+ * The record streams are the file's records in order, not the BAI chunks the reference reads: on a coordinate-sorted file with a correct index
+ * the state machine selects the same reads from either, and this file does not depend on the engine's index code.  -F is not restated here:
+ * the tests apply a Python statement of the query and count the reduced file.
+ *
+ * Library: view_count_oracle(), view_count_oracle_hash(), view_count_oracle_error().  With -DORACLE_MAIN also a CLI:
+ *   view_count_oracle view -c [--num-filter=I1/I2] [-s FRAC] [--subsampling-seed=SEED] [-L BED] in.bam [region ...]
+ * which prints the count as `sambamba view -c` does, or "sambamba-view: <msg>" and exit code 1 for the errors it restates. */
+#include <ctype.h>
+#include <errno.h>
+#include <math.h>
+#include <stdint.h>
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+#include <zlib.h>
+
+static char g_err[512];
+const char* view_count_oracle_error(void) { return g_err; }
+
+typedef struct { int32_t ref, pos; uint16_t flag; int64_t bc; const uint8_t* name; uint32_t l_name; } Rec;
+typedef struct { uint8_t* u; size_t n; int n_ref; char** names; int sorted; Rec* r; size_t nr; } Bam;
+
+static uint32_t rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
+
+static void bam_free(Bam* b) {
+    if (b->names) for (int i = 0; i < b->n_ref; i++) free(b->names[i]);
+    free(b->names); free(b->u); free(b->r); memset(b, 0, sizeof *b);
+}
+
+static int bam_load(const char* path, Bam* b) {
+    memset(b, 0, sizeof *b);
+    gzFile f = gzopen(path, "rb");
+    if (!f) { snprintf(g_err, sizeof g_err, "Cannot open file `%s' in mode `rb' (%s)", path, strerror(errno)); return -1; }
+    size_t cap = 1 << 20; b->u = malloc(cap);
+    for (;;) {
+        if (b->n == cap) { cap *= 2; b->u = realloc(b->u, cap); }
+        int k = gzread(f, b->u + b->n, (unsigned)(cap - b->n > (1u << 30) ? (1u << 30) : cap - b->n));
+        if (k < 0) { int e; snprintf(g_err, sizeof g_err, "DEFLATE error: %s", gzerror(f, &e)); gzclose(f); return -1; }
+        if (k == 0) break;
+        b->n += (size_t)k;
+    }
+    gzclose(f);
+    const uint8_t* u = b->u; size_t n = b->n;
+    if (n < 12 || memcmp(u, "BAM\1", 4)) { snprintf(g_err, sizeof g_err, "Invalid file format: expected BAM\\1"); return -1; }
+    uint32_t l_text = rd32(u + 4); size_t o = 8 + (size_t)l_text;
+    if (o + 4 > n) { snprintf(g_err, sizeof g_err, "truncated BAM header"); return -1; }
+    {   /* @HD SO:coordinate */
+        const char* t = (const char*)u + 8; size_t i = 0;
+        while (i < l_text) {
+            size_t e = i; while (e < l_text && t[e] != '\n') e++;
+            if (e - i >= 3 && !memcmp(t + i, "@HD", 3)) for (size_t k = i; k + 14 <= e; k++) if (!memcmp(t + k, "\tSO:coordinate", 14) && (k + 14 == e || t[k + 14] == '\t')) b->sorted = 1;
+            i = e + 1;
+        }
+    }
+    b->n_ref = (int)rd32(u + o); o += 4;
+    b->names = calloc((size_t)b->n_ref + 1, sizeof(char*));
+    for (int i = 0; i < b->n_ref; i++) {
+        uint32_t ln = rd32(u + o); b->names[i] = malloc(ln + 1); memcpy(b->names[i], u + o + 4, ln); b->names[i][ln] = 0; o += 8 + ln;
+    }
+    size_t rcap = 1024; b->r = malloc(rcap * sizeof(Rec));
+    while (o + 4 <= n) {
+        uint32_t bs = rd32(u + o);
+        if (o + 4 + bs > n) { snprintf(g_err, sizeof g_err, "not enough data in stream"); return -1; }
+        const uint8_t* p = u + o + 4;
+        if (b->nr == rcap) { rcap *= 2; b->r = realloc(b->r, rcap * sizeof(Rec)); }
+        Rec* x = &b->r[b->nr++];
+        x->ref = (int32_t)rd32(p); x->pos = (int32_t)rd32(p + 4);
+        uint32_t bmn = rd32(p + 8), fnc = rd32(p + 12);
+        x->l_name = bmn & 0xFF; x->flag = (uint16_t)(fnc >> 16);
+        uint32_t nc = fnc & 0xFFFF; x->name = p + 32;
+        x->bc = 0;
+        if (!(x->flag & 4)) for (uint32_t k = 0; k < nc; k++) { uint32_t c = rd32(p + 32 + x->l_name + 4 * k), op = c & 15; if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) x->bc += c >> 4; }      /* basesCovered, read.d:255-262 */
+        o += 4 + bs;
+    }
+    if (n - o >= 4) { snprintf(g_err, sizeof g_err, "not enough data in stream"); return -1; }
+    return 0;
+}
+
+uint64_t view_count_oracle_hash(const uint8_t* name, size_t len, uint64_t seed) {
+    uint64_t h = 14695981039346656037ull;
+    for (size_t i = 0; i < len; i++) { h ^= name[i]; h *= 1099511628211ull; }
+    for (int i = 0; i < 8; i++) { h ^= (seed >> (8 * i)) & 0xFF; h *= 1099511628211ull; }
+    return h;
+}
+
+typedef struct { uint32_t ref, start, end; } Reg;
+
+/* BamReadFilter (randomaccessmanager.d:366-462): number of records of rec[0..n) the state machine yields for the sorted, non-overlapping regions. */
+static int keep_read(const Rec* x, unsigned fs, unsigned fu, int sub, uint64_t thr, uint64_t seed) {
+    if ((x->flag & fs) != fs || (x->flag & fu)) return 0;
+    if (sub && (view_count_oracle_hash(x->name, x->l_name ? x->l_name - 1 : 0, seed) & 0xFFFFFFFFull) >= thr) return 0;
+    return 1;
+}
+static uint64_t read_filter_walk(const Bam* b, const Reg* regs, size_t nreg, size_t i0, unsigned fs, unsigned fu, int sub, uint64_t thr, uint64_t seed) {
+    uint64_t cnt = 0; size_t ri = 0; const uint32_t ref_id = regs[0].ref;
+    for (size_t i = i0; i < b->nr && ri < nreg;) {
+        const Rec* x = &b->r[i];
+        uint32_t cur = (uint32_t)x->ref;                          /* cast(uint)ref_id */
+        if (cur > ref_id) break;
+        if (cur < ref_id) { i++; continue; }
+        if ((uint32_t)x->pos >= regs[ri].end) { ri++; continue; }  /* int position against uint end: as unsigned */
+        int yield;
+        if ((uint32_t)x->pos > regs[ri].start) yield = 1;
+        else if ((int64_t)(int32_t)x->pos + x->bc <= (int64_t)regs[ri].start) yield = 0;
+        else yield = 1;
+        if (yield && keep_read(x, fs, fu, sub, thr, seed)) cnt++;
+        i++;
+    }
+    return cnt;
+}
+
+static int cmp_reg(const void* a, const void* b) {
+    const Reg *x = a, *y = b;
+    if (x->ref != y->ref) return x->ref < y->ref ? -1 : 1;
+    if (x->start != y->start) return x->start < y->start ? -1 : 1;
+    return x->end < y->end ? -1 : x->end > y->end;
+}
+
+/* mode 0: every record; 1: -L regions (as parseBed hands them over: any order, merged here as nonOverlappingIntervals does, bed.d:43-58);
+ * 2: positional regions (ref, start, end) in the given order plus n_star '*' queries.  Returns 0 or -1 (view_count_oracle_error()). */
+int view_count_oracle(const char* path, unsigned flag_set, unsigned flag_unset, int subsample, uint64_t threshold, uint64_t seed,
+                      int mode, const uint32_t* regs, size_t nreg, unsigned n_star, uint64_t* out) {
+    Bam b; g_err[0] = 0;
+    if (bam_load(path, &b)) { bam_free(&b); return -1; }
+    uint64_t cnt = 0; int rc = 0;
+    if (mode == 0) {
+        for (size_t i = 0; i < b.nr; i++) cnt += (uint64_t)keep_read(&b.r[i], flag_set, flag_unset, subsample, threshold, seed);
+    } else if (mode == 1) {
+        Reg* r = malloc((nreg + 1) * sizeof(Reg)); size_t m = 0;
+        for (size_t i = 0; i < nreg; i++) if (regs[3 * i + 1] < regs[3 * i + 2]) { r[m].ref = regs[3 * i]; r[m].start = regs[3 * i + 1]; r[m].end = regs[3 * i + 2]; m++; }
+        qsort(r, m, sizeof(Reg), cmp_reg);
+        size_t k = 0;
+        for (size_t i = 0; i < m; i++) { if (k && r[k - 1].ref == r[i].ref && r[k - 1].end >= r[i].start) { if (r[i].end > r[k - 1].end) r[k - 1].end = r[i].end; } else r[k++] = r[i]; }
+        m = k;
+        if (b.sorted) {                                    /* getReadsOverlapping: one BamReadFilter per reference group, joined */
+            for (size_t g = 0; g < m;) { size_t e = g; while (e < m && r[e].ref == r[g].ref) e++; cnt += read_filter_walk(&b, r + g, e - g, 0, flag_set, flag_unset, subsample, threshold, seed); g = e; }
+        } else if (!m) {
+            snprintf(g_err, sizeof g_err, "-L on an unsorted file with no region on the file's references: BedFilter indexes an empty list"); rc = -1;
+        } else {                                           /* BedFilter: trees_.length = bed.back.ref_id + 1 */
+            const uint32_t ntrees = r[m - 1].ref + 1;
+            for (size_t i = 0; i < b.nr; i++) {
+                const Rec* x = &b.r[i];
+                if (x->ref < 0 || (uint32_t)x->ref >= ntrees || !keep_read(x, flag_set, flag_unset, subsample, threshold, seed)) continue;
+                const uint32_t s = (uint32_t)x->pos, t = (uint32_t)((int32_t)x->pos + (int32_t)x->bc);
+                for (size_t j = 0; j < m; j++) if (r[j].ref == (uint32_t)x->ref && r[j].end > s && r[j].start < t) { cnt++; break; }
+            }
+        }
+        free(r);
+    } else {
+        for (size_t i = 0; i < nreg; i++) {
+            Reg one = {regs[3 * i], regs[3 * i + 1], regs[3 * i + 2]};
+            if (!(one.start < one.end)) { snprintf(g_err, sizeof g_err, "start must be less than end"); rc = -1; break; }
+            cnt += read_filter_walk(&b, &one, 1, 0, flag_set, flag_unset, subsample, threshold, seed);
+        }
+        for (unsigned k = 0; k < n_star && !rc; k++) {     /* unmappedReads: the first refID -1 record, then everything to EOF */
+            size_t i = 0; while (i < b.nr && b.r[i].ref != -1) i++;
+            for (; i < b.nr; i++) cnt += (uint64_t)keep_read(&b.r[i], flag_set, flag_unset, subsample, threshold, seed);
+        }
+    }
+    bam_free(&b);
+    if (!rc) *out = cnt;
+    return rc;
+}
+
+#ifdef ORACLE_MAIN
+static int die(const char* m) { fprintf(stderr, "sambamba-view: %s\n", m); return 1; }
+static int conv_u(const char* s, unsigned long long maxv, const char* type, unsigned long long* v) {
+    char m[256];
+    if (!*s) { snprintf(m, sizeof m, "Unexpected end of input when converting from type string to type %s", type); return die(m); }
+    unsigned long long x = 0;
+    for (const char* p = s; *p; p++) {
+        if (*p < '0' || *p > '9') { snprintf(m, sizeof m, "Unexpected '%c' when converting from type string to type %s", *p, type); return die(m); }
+        if (x > (maxv - (unsigned)(*p - '0')) / 10) return die("Conversion positive overflow");
+        x = x * 10 + (unsigned)(*p - '0');
+    }
+    *v = x; return 0;
+}
+/* region.rl: ref[:beg[-end]], 1-based closed -> 0-based half-open */
+static void parse_region(const char* s, char* ref, size_t cap, uint32_t* beg, uint32_t* end) {
+    *beg = 0; *end = UINT32_MAX; size_t n = strlen(s), c = (size_t)-1;
+    for (size_t t = 0; t < n; t++) if (s[t] == ':') {
+        size_t q = t + 1; int ok = q < n && isdigit((unsigned char)s[q]);
+        while (q < n && (isdigit((unsigned char)s[q]) || s[q] == ',')) q++;
+        if (ok && q < n && s[q] == '-') { q++; if (!(q < n && isdigit((unsigned char)s[q]))) ok = 0; while (q < n && (isdigit((unsigned char)s[q]) || s[q] == ',')) q++; }
+        if (ok && q == n) { c = t; break; }
+    }
+    if (c == (size_t)-1) { snprintf(ref, cap, "%s", s); return; }
+    snprintf(ref, cap, "%.*s", (int)c, s);
+    long v = 0; size_t q = c + 1;
+    while (q < n && s[q] != '-') { if (s[q] != ',') v = v * 10 + (s[q] - '0'); q++; }
+    *beg = (uint32_t)(v - 1);
+    if (q < n && s[q] == '-') { q++; v = 0; while (q < n) { if (s[q] != ',') v = v * 10 + (s[q] - '0'); q++; } *end = (uint32_t)v; }
+}
+int main(int argc, char** argv) {
+    if (argc < 2 || strcmp(argv[1], "view")) { fprintf(stderr, "usage: view_count_oracle view -c [options] in.bam [region ...]\n"); return 1; }
+    unsigned long long fs = 0, fu = 0, seed = 0; double frac = NAN; const char* bed = NULL; int count = 0;
+    const char* pos_args[4096]; int npos = 0;
+    for (int i = 2; i < argc; i++) {
+        const char* a = argv[i];
+        if (!strcmp(a, "-c")) count = 1;
+        else if (!strncmp(a, "--num-filter=", 13)) {
+            char buf[256]; snprintf(buf, sizeof buf, "%s", a + 13); char* sl = strchr(buf, '/');
+            if (sl) *sl = 0;
+            if (*buf && conv_u(buf, 0xFFFF, "ushort", &fs)) return 1;
+            if (sl && sl[1] && conv_u(sl + 1, 0xFFFF, "ushort", &fu)) return 1;
+        } else if (!strcmp(a, "-s") && i + 1 < argc) frac = strtod(argv[++i], NULL);
+        else if (!strncmp(a, "--subsampling-seed=", 19)) { if (conv_u(a + 19, 0xFFFFFFFFFFFFFFF0ull, "ulong", &seed)) return 1; }
+        else if (!strcmp(a, "-L") && i + 1 < argc) bed = argv[++i];
+        else if (npos < 4096) pos_args[npos++] = a;
+    }
+    if (!count || npos < 1) { fprintf(stderr, "usage: view_count_oracle view -c [options] in.bam [region ...]\n"); return 1; }
+    int sub = !isnan(frac); uint64_t thr = 0;
+    if (sub) { double t = 4294967296.0 * frac; if (!(t >= 0)) return die("Conversion negative overflow"); if (t > 18446744073709551616.0) return die("Conversion positive overflow"); thr = t >= 18446744073709551616.0 ? UINT64_MAX : (uint64_t)t; }
+    if (bed && npos > 1) return die("specifying both region and BED filename is disallowed");
+    Bam b;
+    if (bam_load(pos_args[0], &b)) { bam_free(&b); return die(g_err); }
+    size_t cap = 1024, n = 0; uint32_t* regs = malloc(cap * 3 * sizeof(uint32_t)); unsigned n_star = 0;
+    int mode = 0;
+    if (bed) {                                             /* readIntervals (bed.d:59-97): whitespace fields, to!long, beg == end -> end + 1, beg < end kept */
+        mode = 1;
+        FILE* f = fopen(bed, "rb"); char msg[600];
+        if (!f) { snprintf(msg, sizeof msg, "%s: %s", bed, strerror(errno)); bam_free(&b); return die(msg); }
+        char line[65536];
+        while (fgets(line, sizeof line, f)) {
+            char* fld[3]; int nf = 0; char* sv = NULL;
+            for (char* t = strtok_r(line, " \t\r\n\v\f", &sv); t && nf < 3; t = strtok_r(NULL, " \t\r\n\v\f", &sv)) fld[nf++] = t;
+            if (nf < 2) continue;
+            long beg = strtol(fld[1], NULL, 10), end = nf >= 3 ? strtol(fld[2], NULL, 10) : beg + 1;
+            if (beg == end) end = beg + 1;
+            if (beg >= end) continue;
+            int id = -1; for (int r = 0; r < b.n_ref; r++) if (!strcmp(b.names[r], fld[0])) id = r;
+            if (id < 0) continue;
+            if (n == cap) { cap *= 2; regs = realloc(regs, cap * 3 * sizeof(uint32_t)); }
+            regs[3 * n] = (uint32_t)id; regs[3 * n + 1] = (uint32_t)beg; regs[3 * n + 2] = (uint32_t)end; n++;
+        }
+        fclose(f);
+    } else if (npos > 1) {
+        mode = 2;
+        for (int i = 1; i < npos; i++) {
+            if (!strcmp(pos_args[i], "*")) { n_star++; continue; }
+            char ref[4096]; uint32_t beg, end; parse_region(pos_args[i], ref, sizeof ref, &beg, &end);
+            int id = -1; for (int r = 0; r < b.n_ref; r++) if (!strcmp(b.names[r], ref)) id = r;
+            if (id < 0) { char msg[4200]; snprintf(msg, sizeof msg, "Reference with name %s does not exist", ref); bam_free(&b); return die(msg); }
+            if (end == UINT32_MAX) {           /* the reference's length from the binary header */
+                size_t o = 8 + rd32(b.u + 4) + 4;
+                for (int r = 0; r < id; r++) o += 8 + rd32(b.u + o);
+                end = rd32(b.u + o + 4 + rd32(b.u + o));
+            }
+            if (!(beg < end)) { bam_free(&b); return die("start must be less than end"); }
+            if (n == cap) { cap *= 2; regs = realloc(regs, cap * 3 * sizeof(uint32_t)); }
+            regs[3 * n] = (uint32_t)id; regs[3 * n + 1] = beg; regs[3 * n + 2] = end; n++;
+        }
+    }
+    bam_free(&b);
+    uint64_t cnt = 0;
+    if (view_count_oracle(pos_args[0], (unsigned)fs, (unsigned)fu, sub, thr, seed, mode, regs, n, n_star, &cnt)) { free(regs); return die(g_err); }
+    free(regs);
+    printf("%llu\n", (unsigned long long)cnt);
+    return 0;
+}
+#endif
