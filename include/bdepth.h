@@ -23,6 +23,8 @@
  *   computeFlagStatistics(bam.reads)     sambamba/flagstat.d:31-57,127   bdepth_run_flagstat (`sambamba flagstat`)
  *   ReadCounter over view_main's reads   sambamba/view.d:265-379,        bdepth_run_view_count (`sambamba view -c`)
  *     (filters, -L, regions, '*')        utils/view/alignmentrangeprocessor.d:42-50
+ *   SamSerializer over view_main's reads sambamba/view.d:265-379,        bdepth_run_view_text (`sambamba view`, SAM lines)
+ *     (BamRead.toSam per read)           utils/view/alignmentrangeprocessor.d:97-106
  *
  * Conventions: every entry returns 0 on success or a negative bdepth_status; the message is
  * available through bdepth_last_error().  No exception crosses the boundary.  There is no CPU
@@ -283,6 +285,20 @@ typedef struct {
  * Several ranks: each counts its shard (or its share of the region chunks) and one all-reduce sums the counts; a rank that fails makes every rank
  * return BDEPTH_ERR_NCCL.  Malformed input is BDEPTH_ERR_FORMAT as in every run.  Timings: ms_inflate, ms_scan and, for k_view_count, ms_reduce. */
 int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* opts, uint64_t* count);
+/* In a BDEPTH_VIEW_POSITIONAL region list of bdepth_run_view_text: the region argument '*' (unmappedReads) at that place of the list. */
+#define BDEPTH_VIEW_UNMAPPED 0xFFFFFFFFu
+/* `sambamba view` without -c, -h or -H: exactly what SamSerializer (utils/view/alignmentrangeprocessor.d:97-106) writes after the header, which
+ * stays with the host.  One line per read: BamRead.toSam (read.d:695-760) plus '\n'.  The selection and options are bdepth_run_view_count's; the
+ * order is the reference's joined stream (view.d:308-366): file order without regions and with -L; positional regions one argument after the
+ * other, in the order given (one pipeline run each; a region given twice prints twice; ref_id BDEPTH_VIEW_UNMAPPED is '*' in its place, and
+ * n_unmapped must be 0).  cb gets whole lines, in order, from pinned memory reused once it returns (pieces of at most 64 MB or one batch of text,
+ * plus one line); non-zero stops the run with BDEPTH_ERR_CALLBACK.  BDEPTH_ERR_FORMAT where the reference throws or indexes out of bounds: a refID
+ * or next refID outside [-1, n_ref) where a name is printed, an unknown tag or B element type, a Z / H value without its NUL, a tag or B array
+ * running past the record; also an index found not to describe a sorted file after lines went out.  Several ranks (no regions, -L): each delivers
+ * its own records' lines, the texts joined in rank order are the single-GPU text, and a final all-reduce of a failure word tells every rank that
+ * the join is complete (BDEPTH_ERR_NCCL otherwise); positional regions there, and bdepth_add_input handles, are BDEPTH_ERR_ARG.
+ * Timings: ms_inflate, ms_scan, ms_reduce (formatting kernels), ms_d2h (text copies), summed over the runs of a positional query. */
+int bdepth_run_view_text(bdepth_t* h, const bdepth_view_opts* opts, bdepth_text_cb cb, void* user);
 /* Scan records on the GPU; copy out up to cap rows of the columnar SoA (any pointer may be NULL). */
 int64_t bdepth_scan_to_host(bdepth_t* h, uint64_t cap, int32_t* ref_id, int32_t* pos, uint32_t* span, uint16_t* flag, uint8_t* mapq, uint16_t* n_cigar, uint64_t* rec_off);
 

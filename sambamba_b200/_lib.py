@@ -143,6 +143,7 @@ def load_library():
     L.bdepth_build_index.restype = C.c_int64
     L.bdepth_run_flagstat.argtypes = [vp, C.POINTER(FlagStat)]
     L.bdepth_run_view_count.argtypes = [vp, C.POINTER(ViewOpts), C.POINTER(C.c_uint64)]
+    L.bdepth_run_view_text.argtypes = [vp, C.POINTER(ViewOpts), TEXT_CB, vp]
     _lib = L
     return L
 
@@ -153,7 +154,7 @@ EXPORTED_SYMBOLS = [
     "bdepth_n_samples", "bdepth_sample_name", "bdepth_set_filter", "bdepth_set_filter_query", "bdepth_set_min_baseq", "bdepth_set_fix_mates", "bdepth_set_combined", "bdepth_set_regions",
     "bdepth_set_shard", "bdepth_nccl_unique_id", "bdepth_plan_shards", "bdepth_plan_region_chunks", "bdepth_set_tuning", "bdepth_stage", "bdepth_run_resident", "bdepth_run_base", "bdepth_run_base_text",
     "bdepth_run_windows", "bdepth_run_regions", "bdepth_get_stats", "bdepth_ref_has_reads", "bdepth_inflate_to_host", "bdepth_scan_to_host", "bdepth_build_index",
-    "bdepth_run_flagstat", "bdepth_run_view_count",
+    "bdepth_run_flagstat", "bdepth_run_view_count", "bdepth_run_view_text",
 ]
 
 
@@ -407,21 +408,47 @@ class BDepth:
         self._ck(self.L.bdepth_run_flagstat(self.h, C.byref(fs)))
         return fs.as_dict()
 
-    def run_view_count(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, n_unmapped=0):
-        """`sambamba view -c`: the number of selected reads.  num_filter = (i1, i2); subsample = fraction (with `seed`); bed = [(ref, beg, end)]
-        as -L; regions = [(ref, beg, end)] positional queries, plus n_unmapped '*' queries."""
+    @staticmethod
+    def _view_opts(num_filter, query, subsample, seed, bed, regions, n_unmapped=0):
         o = ViewOpts()
         o.flag_set, o.flag_unset = num_filter
         o.query = query.encode() if query is not None else None
         if subsample is not None:
             o.subsample, o.subsample_threshold, o.subsampling_seed = 1, subsample_threshold(subsample), seed
-        rg = bed if bed is not None else (regions or [])
-        arr = (Region * max(len(rg), 1))(*[Region(*r) for r in rg])
+        rg = [(0xFFFFFFFF, 0, 0) if r == "*" else r for r in (bed if bed is not None else (regions or []))]      # "*": BDEPTH_VIEW_UNMAPPED
+        o._arr = (Region * max(len(rg), 1))(*[Region(*r) for r in rg])
         o.regions_from = 1 if bed is not None else 2 if (rg or n_unmapped) else 0      # BDEPTH_VIEW_BED / _POSITIONAL / _ALL
-        o.regions, o.n_regions, o.n_unmapped = arr, len(rg), n_unmapped
+        o.regions, o.n_regions, o.n_unmapped = o._arr, len(rg), n_unmapped
+        return o
+
+    def run_view_count(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, n_unmapped=0):
+        """`sambamba view -c`: the number of selected reads.  num_filter = (i1, i2); subsample = fraction (with `seed`); bed = [(ref, beg, end)]
+        as -L; regions = [(ref, beg, end)] positional queries, plus n_unmapped '*' queries."""
         n = C.c_uint64()
-        self._ck(self.L.bdepth_run_view_count(self.h, C.byref(o), C.byref(n)))
+        self._ck(self.L.bdepth_run_view_count(self.h, C.byref(self._view_opts(num_filter, query, subsample, seed, bed, regions, n_unmapped)), C.byref(n)))
         return n.value
+
+    def run_view_text(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, sink=None):
+        """`sambamba view`: the SAM lines of the selected reads (no header).  The keywords are run_view_count's; `regions` may hold "*" entries,
+        each the region argument '*' in its place.  Returns the text, or hands each chunk to sink(bytes) and returns the number of bytes; a sink
+        that raises stops the run (BDepthError BDEPTH_ERR_CALLBACK, the sink's exception as its cause)."""
+        parts, total, err = [], [0], []
+
+        def cb(_user, ptr, n):
+            try:
+                (parts.append if sink is None else sink)(C.string_at(ptr, n))
+                total[0] += n
+                return 0
+            except BaseException as e:  # noqa: BLE001 -- handed back to the caller after the run
+                err.append(e)
+                return 1
+        try:
+            self._ck(self.L.bdepth_run_view_text(self.h, C.byref(self._view_opts(num_filter, query, subsample, seed, bed, regions)), TEXT_CB(cb), None))
+        except BDepthError as e:
+            if err:
+                raise e from err[0]
+            raise
+        return total[0] if sink is not None else b"".join(parts)
 
     def scan(self, cap):
         cols = dict(ref_id=np.zeros(cap, np.int32), pos=np.zeros(cap, np.int32), span=np.zeros(cap, np.uint32),

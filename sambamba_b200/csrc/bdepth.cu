@@ -80,7 +80,7 @@ constexpr size_t EMIT_CHUNK = 4ull << 20;     // positions per D2H chunk
 constexpr uint32_t SHARD_EXTRA_BLOCKS = 8;
 constexpr uint32_t MATE_ZONE_BLOCKS = 64;       // -m on several ranks: blocks read behind the shard so that pairs cut by the boundary are seen whole
 
-enum RunMode { RUN_FULL = 0, RUN_INFLATE_ONLY = 1, RUN_SCAN_ONLY = 2, RUN_INDEX = 3, RUN_FLAGSTAT = 4, RUN_VIEW_COUNT = 5 };
+enum RunMode { RUN_FULL = 0, RUN_INFLATE_ONLY = 1, RUN_SCAN_ONLY = 2, RUN_INDEX = 3, RUN_FLAGSTAT = 4, RUN_VIEW_COUNT = 5, RUN_VIEW_TEXT = 6 };
 constexpr int RC_RETRY_WINDOW = 1;      // internal: a read lies outside the counter window a multi-input run was given
 
 // ---- NCCL, bound at run time (dlopen) so that single-GPU users need no NCCL at all and so that a host
@@ -203,6 +203,17 @@ struct bdepth {
     DevBuf fs; uint64_t fs_host[FS_WORDS + 1] = {};
     // ---- view -c (bdepth_run_view_count): the selection of the current run, its device tables, the count plus a "failed rank" word and their host copy
     ViewSel vsel{}; DevBuf vc, vc_reg, vc_prog; uint64_t vc_host[2] = {};
+    // ---- view's SAM lines (bdepth_run_view_text): per sub-batch the line lengths, their offsets and the piece cuts; two text slots on the device
+    // and their pinned host copies (one is handed to the callback while the next piece is written and copied); timings of the run
+    struct ViewText {
+        bdepth_text_cb cb = nullptr; void* user = nullptr;
+        DevBuf names, len, off, tiles, ctl, cut_r, cut_o, slot[2];
+        char* host = nullptr; size_t cap = 0;          // bytes per slot (device and host)
+        bool pend[2] = {false, false}; size_t pend_len[2] = {0, 0}; int next = 0;
+        uint64_t issued = 0;                           // bytes handed to the D2H in the current pipeline run
+        float ms_fmt = 0, ms_d2h = 0;
+        SamTab tab{};                                  // the reference names on the device (ctl is set per sub-batch)
+    } vt;
     // ---- several BAM files (bdepth_add_input; MultiBamReader, multireader.d:218-268): the additional files are whole handles that
     // only hold their input (file, BGZF members, header, index, shard / sparse plan); a run swaps them into this handle one after
     // the other and accumulates into the same counters -- per-position counters and per-segment sums are additive over reads,
@@ -637,6 +648,88 @@ struct RunOut {                    // optional sinks for the kernel-level entry 
 
 __global__ void k_fill_u32(uint32_t* p, uint32_t v, uint64_t n) { uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; if (i < n) p[i] = v; }
 
+// ---- view's SAM lines (RUN_VIEW_TEXT).  Per sub-batch, while its records are still in the inflate buffer: k_sam_len measures the line of every
+// selected record, a device-wide scan turns the lengths into offsets, one small copy brings the total, the longest line and the error word down,
+// and k_sam_cut cuts the records into pieces of about VIEW_TEXT_PIECE bytes of text (a piece always holds whole lines, so a slot holds a piece plus
+// the longest line).  Each piece is written by k_sam_write into a device slot and copied into pinned memory on the D2H stream; the callback
+// gets a slot while the next piece is written and copied into the other.
+constexpr uint64_t VIEW_TEXT_PIECE = 64ull << 20;     // capped by the batch size (bdepth_set_tuning), so that small batches make many pieces
+const char* sam_err_msg(unsigned long long c) {
+    switch (c) {
+        case SAM_ERR_REF: return "a record's reference ID lies outside [-1, n_ref): no RNAME to print (the reference indexes its reference list out of bounds)";
+        case SAM_ERR_MATE_REF: return "a record's mate reference ID lies outside [-1, n_ref): no RNEXT to print (the reference indexes its reference list out of bounds)";
+        case SAM_ERR_TAG_TYPE: return "unknown tag type in a record's auxiliary data (UnknownTagTypeException)";
+        case SAM_ERR_B_TYPE: return "unknown element type of a B array in a record's auxiliary data (UnknownTagTypeException)";
+        case SAM_ERR_NO_NUL: return "a Z or H tag value without its terminating NUL";
+        default: return "a record's fields, a tag or a B array run past the record's block_size";
+    }
+}
+int view_text_deliver(bdepth* h, int slot) {
+    auto& V = h->vt;
+    if (!V.pend[slot]) return 0;
+    CK(cudaEventSynchronize(h->ev[26 + slot])); V.pend[slot] = false;
+    float t = 0; CK(cudaEventElapsedTime(&t, h->ev[28 + slot], h->ev[24 + slot])); V.ms_fmt += t;
+    CK(cudaEventElapsedTime(&t, h->ev[24 + slot], h->ev[26 + slot])); V.ms_d2h += t;
+    if (V.cb && V.pend_len[slot] && V.cb(V.user, V.host + (size_t)slot * V.cap, V.pend_len[slot])) return fail(h, BDEPTH_ERR_CALLBACK, "text callback aborted");
+    return 0;
+}
+int view_text_flush(bdepth* h) { int rc = view_text_deliver(h, h->vt.next); if (!rc) rc = view_text_deliver(h, h->vt.next ^ 1); return rc; }
+int view_text_sub(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R, int64_t own_from) {
+    auto& V = h->vt; cudaStream_t sm = h->s_main;
+    const uint32_t n_tiles = (R + SAM_SCAN_TILE - 1) / SAM_SCAN_TILE;
+    const size_t toff_at = ((size_t)n_tiles * 4 + 7) / 8 * 8;
+    CK(V.len.ensure((size_t)R * 4)); CK(V.off.ensure((size_t)R * 8)); CK(V.tiles.ensure(toff_at + (size_t)n_tiles * 8)); CK(V.ctl.ensure(32));
+    uint32_t* len = V.len.as<uint32_t>(); unsigned long long* off = V.off.as<unsigned long long>();
+    uint32_t* tsum = V.tiles.as<uint32_t>(); unsigned long long* toff = (unsigned long long*)(V.tiles.as<uint8_t>() + toff_at);
+    SamTab t = V.tab; t.ctl = V.ctl.as<unsigned long long>();
+    CK(cudaMemsetAsync(t.ctl, 0, 24, sm));
+    CK(cudaEventRecord(h->ev[30], sm));
+    BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_sam_len)(soa, u0, R, own_from, h->vsel, t, len);
+    BD_LAUNCH(n_tiles, 256, 0, sm, k_sam_tile_sum)(len, R, tsum);
+    BD_LAUNCH(1, 1024, 0, sm, k_text_scan)(tsum, n_tiles, toff, t.ctl);
+    BD_LAUNCH(n_tiles, 256, 0, sm, k_sam_scan_apply)(len, R, toff, off);
+    CK(cudaGetLastError()); h->st.gpu_launches += 4;
+    CK(cudaEventRecord(h->ev[31], sm));
+    unsigned long long c[3]; CK(cudaMemcpyAsync(c, t.ctl, 24, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
+    { float tm = 0; CK(cudaEventElapsedTime(&tm, h->ev[30], h->ev[31])); V.ms_fmt += tm; }
+    if (c[2]) return fail(h, BDEPTH_ERR_FORMAT, "%s", sam_err_msg(c[2]));
+    const uint64_t total = c[0];
+    if (!total) return 0;
+    const uint64_t piece = std::max<uint64_t>(1, std::min<uint64_t>(VIEW_TEXT_PIECE, h->batch_u));
+    if (piece + c[1] > V.cap) {      // a slot holds a piece and its longest line: grow both, after handing out what is pending in them
+        int rc = view_text_flush(h); if (rc) return rc;
+        if (V.host) { cudaFreeHost(V.host); V.host = nullptr; }
+        V.cap = 0;
+        const size_t need = piece + std::max<uint64_t>(c[1], piece);
+        CK(cudaMallocHost((void**)&V.host, 2 * need)); CK(V.slot[0].ensure(need)); CK(V.slot[1].ensure(need));
+        V.cap = need;
+    }
+    const uint32_t n_cuts = (uint32_t)((total + piece - 1) / piece) + 1;
+    CK(V.cut_r.ensure((size_t)n_cuts * 4)); CK(V.cut_o.ensure((size_t)n_cuts * 8));
+    BD_LAUNCH((n_cuts + 255) / 256, 256, 0, sm, k_sam_cut)(off, R, total, piece, n_cuts, V.cut_r.as<uint32_t>(), V.cut_o.as<unsigned long long>());
+    CK(cudaGetLastError()); h->st.gpu_launches++;
+    std::vector<uint32_t> cr(n_cuts); std::vector<unsigned long long> co(n_cuts);
+    CK(cudaMemcpyAsync(cr.data(), V.cut_r.p, (size_t)n_cuts * 4, cudaMemcpyDeviceToHost, sm)); CK(cudaMemcpyAsync(co.data(), V.cut_o.p, (size_t)n_cuts * 8, cudaMemcpyDeviceToHost, sm));
+    CK(cudaStreamSynchronize(sm));
+    for (uint32_t j = 0; j + 1 < n_cuts; j++) {
+        const uint32_t r0 = cr[j], r1 = j + 2 == n_cuts ? R : cr[j + 1];
+        const uint64_t bytes = (j + 2 == n_cuts ? total : co[j + 1]) - co[j];
+        if (!bytes) continue;
+        const int s = V.next;
+        int rc = view_text_deliver(h, s); if (rc) return rc;      // the slot's previous piece must be consumed before reuse
+        CK(cudaEventRecord(h->ev[28 + s], sm));
+        BD_LAUNCH((unsigned)std::min<uint64_t>((r1 - r0 + 7) / 8, 8192), 256, 0, sm, k_sam_write)(soa.off, u0, r0, r1, len, off, t, V.slot[s].as<char>());
+        CK(cudaGetLastError()); h->st.gpu_launches++;
+        CK(cudaEventRecord(h->ev[24 + s], sm));
+        CK(cudaStreamWaitEvent(h->s_d2h, h->ev[24 + s], 0));
+        CK(cudaMemcpyAsync(V.host + (size_t)s * V.cap, V.slot[s].p, bytes, cudaMemcpyDeviceToHost, h->s_d2h));
+        CK(cudaEventRecord(h->ev[26 + s], h->s_d2h));
+        V.pend[s] = true; V.pend_len[s] = bytes; V.issued += bytes; V.next = s ^ 1;
+        rc = view_text_deliver(h, s ^ 1); if (rc) return rc;     // hand out the previous piece while this one is in flight
+    }
+    return 0;
+}
+
 // The pipeline: leaves the per-position counters of the whole shard in h->counts (RUN_FULL).
 int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em);
 int run_pipeline(bdepth* h, RunMode mode, RunOut* ro, Emitter* em = nullptr) {
@@ -650,8 +743,10 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     auto t_host0 = std::chrono::steady_clock::now();
     bdepth_stats& st = h->st; uint32_t launches0 = 0;
     st = bdepth_stats{}; st.gpu_launches = launches0;
-    const bool sparse = (mode == RUN_FULL || mode == RUN_VIEW_COUNT) && plan_sparse(h);      // (view -c: bdepth_run_view_count has put its own regions there)
-    h->coll_pending = (mode == RUN_FULL && h->world > 1 && h->comm) ? (sparse ? 2 : 1) : (mode == RUN_FLAGSTAT && h->world > 1 && h->comm) ? 3 : (mode == RUN_VIEW_COUNT && h->world > 1 && h->comm) ? (sparse ? 2 : 4) : 0;
+    const bool view = mode == RUN_VIEW_COUNT || mode == RUN_VIEW_TEXT;      // view's selection: its count, or its SAM lines
+    if (mode == RUN_VIEW_TEXT) { h->vt.issued = 0; h->vt.ms_fmt = h->vt.ms_d2h = 0; }
+    const bool sparse = (mode == RUN_FULL || view) && plan_sparse(h);      // (view: bdepth_run_view_count / _text has put its own regions there)
+    h->coll_pending = (mode == RUN_FULL && h->world > 1 && h->comm) ? (sparse ? 2 : 1) : (mode == RUN_FLAGSTAT && h->world > 1 && h->comm) ? 3 : (view && h->world > 1 && h->comm) ? (sparse ? 2 : 4) : 0;
     if (!sparse) { rc = prepare_shard(h); if (rc) return rc; }      // the plain path needs the whole file's member table (a lazily opened handle frames it now)
     // -m pairs reads of one name wherever they sit in the shard.  A batch is scanned as a whole (no sub-batches), and every
     // batch after the first re-reads the end of the previous one as "ghost" records -- from the earliest record that can
@@ -716,7 +811,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     }
     CK(h->scan_stats.ensure(sizeof(ScanStats)));
     const FilterProg* d_fprog = nullptr;
-    if (h->has_fprog && mode != RUN_FLAGSTAT && mode != RUN_VIEW_COUNT) { CK(h->fprog_d.ensure(sizeof(FilterProg))); CK(cudaMemcpyAsync(h->fprog_d.p, &h->fprog, sizeof(FilterProg), cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm)); d_fprog = h->fprog_d.as<FilterProg>(); }
+    if (h->has_fprog && mode != RUN_FLAGSTAT && !view) { CK(h->fprog_d.ensure(sizeof(FilterProg))); CK(cudaMemcpyAsync(h->fprog_d.p, &h->fprog, sizeof(FilterProg), cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm)); d_fprog = h->fprog_d.as<FilterProg>(); }
     RgTable rgt{nullptr, nullptr, nullptr, 0};
     if (mode == RUN_FULL && (h->S > 1 || (fix && h->hdr.sample_names.size() > 1))) {      // @RG ID -> sample table for the per-read RG lookup (depth.d:240-250); mates pair within a sample
         std::vector<uint8_t> ids; std::vector<uint32_t> offs; std::vector<uint8_t> samp;
@@ -765,7 +860,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     }
     float ms_census = 0;
     if (mode == RUN_FLAGSTAT) { CK(h->fs.ensure((FS_WORDS + 1) * 8)); CK(cudaMemsetAsync(h->fs.p, 0, (FS_WORDS + 1) * 8, sm)); }
-    if (mode == RUN_VIEW_COUNT) { CK(h->vc.ensure(16)); CK(cudaMemsetAsync(h->vc.p, 0, 16, sm)); }
+    if (view) { CK(h->vc.ensure(16)); CK(cudaMemsetAsync(h->vc.p, 0, 16, sm)); }
     CK(cudaEventRecord(h->ev[10], sm));
     size_t b = blk_lo;
     if (ro) { ro->inflate_len = 0; ro->scan_n = 0; }
@@ -901,7 +996,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
                 CK(cudaEventRecord(h->k1_ev[j], ks));
                 // Sub-batches: a lane needs ~60 ms for its block however empty the GPU is, so the scan / coverage /
                 // delivery of the blocks that arrived first runs while the later chunks are still being inflated.
-                if ((mode == RUN_FULL || mode == RUN_INDEX || mode == RUN_FLAGSTAT || mode == RUN_VIEW_COUNT) && !fix) subs.push_back(Sub{c0, c1, (int)j, (int)j}); else { if (subs.empty()) subs.push_back(Sub{b, b1, 0, (int)j}); subs[0].ev_hi = (int)j; }
+                if ((mode == RUN_FULL || mode == RUN_INDEX || mode == RUN_FLAGSTAT || view) && !fix) subs.push_back(Sub{c0, c1, (int)j, (int)j}); else { if (subs.empty()) subs.push_back(Sub{b, b1, 0, (int)j}); subs[0].ev_hi = (int)j; }
                 c0 = c1;
             }
         }
@@ -995,7 +1090,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
                         // the index does not describe this file (the reference only checks that one exists): plain pass instead.
                         // On several ranks that decision has to be taken by all of them together (below, after the batches):
                         // a rank falling back on its own would leave the union of the ranks' records no partition of the file.
-                        if (h->world == 1) { h->sparse_ok = false; CK(cudaDeviceSynchronize()); return run_pipeline(h, mode, ro, em); }
+                        if (h->world == 1) { if (mode == RUN_VIEW_TEXT && h->vt.issued) return fail(h, BDEPTH_ERR_FORMAT, "the index does not describe this file (a region chunk does not end at a record), found after SAM lines were delivered"); h->sparse_ok = false; CK(cudaDeviceSynchronize()); return run_pipeline(h, mode, ro, em); }
                         sparse_bad = true; break;
                     }
                     cur = INT64_MAX / 2;                                  // nothing follows until the next chunk begins
@@ -1042,7 +1137,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         const int64_t own_hi = (fix && h->world > 1 && h->limit_abs_u < h->total_u) ? (int64_t)h->limit_abs_u - (int64_t)batch_u0 : INT64_MAX;
         const int64_t zone_below = (!fix && !sparse && h->world > 1) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;       // records of the previous ranks' zone
         UP(h->scan_stats.p, &zs, sizeof zs);
-        if ((mode == RUN_SCAN_ONLY || mode == RUN_INDEX || mode == RUN_FLAGSTAT || mode == RUN_VIEW_COUNT) && !h->ref_has.p) { CK(h->ref_has.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has.p, 0, (nref / 32 + 2) * 4, sm)); }
+        if ((mode == RUN_SCAN_ONLY || mode == RUN_INDEX || mode == RUN_FLAGSTAT || view) && !h->ref_has.p) { CK(h->ref_has.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has.p, 0, (nref / 32 + 2) * 4, sm)); }
         // runs with -L regions: K2's every-passing-read bits go to a scratch word array, k_ref_seen marks the references of the reads that overlap a region
         uint32_t* has_dst = h->ref_has.as<uint32_t>();
         const uint32_t n_flt_k2 = mode == RUN_FULL ? (uint32_t)h->regions.size() : 0u;
@@ -1063,7 +1158,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         else K2_DECODE(false, false);
 #undef K2_DECODE
         CK(cudaGetLastError()); st.gpu_launches++;
-        if (R && mode != RUN_INDEX && mode != RUN_SCAN_ONLY && mode != RUN_FLAGSTAT && mode != RUN_VIEW_COUNT) {      // quirk 1: CIGARs that begin with N, rewritten to what the reference's cursor makes of them (the index, the raw scan, flagstat and view -c see the file as it is)
+        if (R && mode != RUN_INDEX && mode != RUN_SCAN_ONLY && mode != RUN_FLAGSTAT && !view) {      // quirk 1: CIGARs that begin with N, rewritten to what the reference's cursor makes of them (the index, the raw scan, flagstat and view see the file as it is)
             // region mode proper (no window slots, no -m, one rank): the statistics of such a read are reproduced (kernels.cuh); otherwise refused
             const bool lead_n_regions = h->seg.on && h->seg.n && !h->seg.has_u && !h->seg.has_min && !fix && h->world == 1;
             LeadNSegs lsg{nullptr, nullptr, nullptr, nullptr, 0u, nullptr, nullptr, 1u, h->minq};
@@ -1239,6 +1334,11 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             CK(cudaGetLastError()); st.gpu_launches++;
             CK(cudaEventRecord(h->ev[23], sm));
         }
+        // ---- view: the SAM lines of the sub-batch's selected records, handed out before the inflate buffer is reused
+        if (mode == RUN_VIEW_TEXT && R) {
+            const int64_t own_from = (h->world > 1 && !sparse) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;
+            rc = view_text_sub(h, soa, u0, (uint32_t)R, own_from); if (rc) return rc;
+        }
         // Progressive delivery: positions below the start of the sub-batch's last own read are final (the file is coordinate sorted).  Several ranks
         // (plain shards): a rank's own positions begin at its first passing read -- known once such a read has been seen -- and the reads of the
         // previous ranks that reach into them come first in its stream (the zone), so the same holds; where its positions end it learns at the end.
@@ -1268,11 +1368,12 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             uint32_t flag = sparse_bad ? 1u : 0u;
             CK(cudaMemcpyAsync(h->misc.p, &flag, 4, cudaMemcpyHostToDevice, sm));
             NK(nccl().AllReduce(h->misc.p, h->misc.p, 1, NCCL_UINT32, NCCL_SUM, h->comm, sm));
-            h->coll_pending = mode == RUN_VIEW_COUNT ? 4 : 1;
+            h->coll_pending = view ? 4 : 1;
             CK(cudaMemcpyAsync(&flag, h->misc.p, 4, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
             if (flag >= SPARSE_PEER_FAILED) { h->coll_pending = 0; return fail(h, BDEPTH_ERR_NCCL, "another rank of the run stopped with an error (its own message says why): no result"); }
             sparse_bad = flag != 0;
         } else if (sparse_bad) return fail(h, BDEPTH_ERR_FORMAT, "the index does not describe this file (a region chunk does not end at a record); several ranks without a NCCL id cannot fall back together");
+        if (sparse_bad && mode == RUN_VIEW_TEXT) { h->coll_pending = 4; return fail(h, BDEPTH_ERR_FORMAT, "the index does not describe this file (a region chunk does not end at a record), found after SAM lines were delivered"); }
         if (sparse_bad) { h->sparse_ok = false; CK(cudaDeviceSynchronize()); return run_pipeline(h, mode, ro, em); }
     }
     st.ms_h2d = ms_h2d; st.ms_inflate = ms_k1; st.ms_scan = ms_k2; st.ms_coverage = ms_k3;
@@ -1285,14 +1386,15 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         if (h->fs_host[FS_WORDS]) return fail(h, BDEPTH_ERR_NCCL, "another rank of the run stopped with an error (its own message says why): no result");
         st.ms_reduce = ms_census;
     }
-    if (mode == RUN_VIEW_COUNT) {      // several ranks: one all-reduce of the count and the "failed" word (abort_collectives), as for flagstat
+    if (mode == RUN_VIEW_TEXT) { rc = view_text_flush(h); if (rc) return rc; st.ms_d2h = h->vt.ms_d2h; }      // the last piece, before the ranks learn that this one is complete
+    if (view) {      // several ranks: one all-reduce of the count and the "failed" word (abort_collectives), as for flagstat
         if (h->world > 1 && h->comm) { NK(nccl().AllReduce(h->vc.p, h->vc.p, 2, NCCL_UINT64, NCCL_SUM, h->comm, sm)); h->coll_pending = 0; }
         CK(hs.ensure(16384)); hs.used = 0;
         DOWN(vcp, uint64_t, h->vc.p, 16);
         CK(cudaStreamSynchronize(sm));
         memcpy(h->vc_host, vcp, sizeof h->vc_host);
         if (h->vc_host[1]) return fail(h, BDEPTH_ERR_NCCL, "another rank of the run stopped with an error (its own message says why): no result");
-        st.ms_reduce = ms_census;
+        st.ms_reduce = mode == RUN_VIEW_TEXT ? h->vt.ms_fmt : ms_census;
     }
     st.positions = mode == RUN_FULL ? h->hdr.total_len : 0;
     h->own_lo = 0; h->own_hi = h->hdr.total_len;
@@ -1478,6 +1580,7 @@ void bdepth_close(bdepth_t* h) {
     { auto& X = h->ix; X.lin.release(); X.lin_len.release(); X.lin_base.release(); X.lin_cap.release(); X.n_mapped.release(); X.n_unmapped.release(); X.carry.release(); X.ctl.release(); X.runs.release(); X.excs.release(); }
     h->m_hash.release(); h->m_flag.release(); h->m_flt.release(); h->m_ctl.release(); h->fprog_d.release();
     h->vc.release(); h->vc_reg.release(); h->vc_prog.release();
+    { auto& V = h->vt; V.names.release(); V.len.release(); V.off.release(); V.tiles.release(); V.ctl.release(); V.cut_r.release(); V.cut_o.release(); V.slot[0].release(); V.slot[1].release(); if (V.host) cudaFreeHost(V.host); V.host = nullptr; V.cap = 0; }
     if (h->comm) { nccl().CommDestroy(h->comm); h->comm = nullptr; }
     if (h->pinned) cudaFreeHost(h->pinned);
     h->hs.release();
@@ -2022,13 +2125,12 @@ int bdepth_run_flagstat(bdepth_t* h, bdepth_flagstat* out) {
 // ReadCounter over view_main's selection (sambamba/view.d:265-368): K1 + K2 as in every run, then k_view_count per sub-batch.  Regions on a
 // coordinate-sorted file with a usable index stage only their BAI chunks (plan_sparse, with the view's regions in place of the handle's for the
 // duration of the run); otherwise every record of the file is scanned.  The handle's depth settings are not used and stay as they were.
-int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* o, uint64_t* count) {
-    if (!h) return BDEPTH_ERR_ARG;
-    if (!o || !count || (o->n_regions && !o->regions)) return fail(h, BDEPTH_ERR_ARG, "null argument");
-    if (o->regions_from < BDEPTH_VIEW_ALL || o->regions_from > BDEPTH_VIEW_POSITIONAL) return fail(h, BDEPTH_ERR_ARG, "regions_from: %d", o->regions_from);
+// The selection of one view run into h->vsel and what to stage into `plan`: the flag bits, -s, -F from o, the regions regs[0, n_regs) read as
+// o->regions_from says, and n_star '*' queries.  *empty: the run selects nothing (-L naming no region of a sorted file).
+int view_setup(bdepth* h, const bdepth_view_opts* o, const bdepth_region* regs, size_t n_regs, uint32_t n_star, std::vector<bdepth_region>& plan, bool* empty) {
     const bool positional = o->regions_from == BDEPTH_VIEW_POSITIONAL;
-    if (!h->extra.empty()) return fail(h, BDEPTH_ERR_ARG, "view reads one BAM file: this handle has several inputs (bdepth_add_input)");
     const size_t nref = h->hdr.ref_len.size();
+    *empty = false;
     ViewSel vs{}; vs.flag_set = o->flag_set; vs.flag_unset = o->flag_unset;
     vs.subsample = o->subsample ? 1u : 0u; vs.threshold = o->subsample_threshold; vs.seed = o->subsampling_seed;
     FilterProg prog; bool has_prog = false;
@@ -2039,24 +2141,24 @@ int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* o, uint64_t* coun
         has_prog = true;
     }
     std::vector<bdepth_region> rg;
-    for (size_t i = 0; i < o->n_regions; i++) {
-        const bdepth_region& g = o->regions[i];
+    for (size_t i = 0; i < n_regs; i++) {
+        const bdepth_region& g = regs[i];
         if (g.ref_id >= nref) return fail(h, BDEPTH_ERR_ARG, "region #%zu: reference %u out of range", i, g.ref_id);
         if (g.start >= g.end) { if (positional) return fail(h, BDEPTH_ERR_ARG, "start must be less than end"); continue; }      // opSlice, reference.d:77; parseBed keeps beg < end only
         rg.push_back(g);
     }
     const bool sorted = h->hdr.so_coordinate;
-    if (positional) vs.region_mode = (rg.empty() && !o->n_unmapped) ? VIEW_ALL : VIEW_POSITIONAL;
+    if (positional) vs.region_mode = (rg.empty() && !n_star) ? VIEW_ALL : VIEW_POSITIONAL;
     else vs.region_mode = o->regions_from == BDEPTH_VIEW_BED ? VIEW_MERGED : VIEW_ALL;
-    vs.n_star = positional ? o->n_unmapped : 0;
+    vs.n_star = positional ? n_star : 0;
     if (vs.region_mode == VIEW_MERGED && rg.empty()) {
         if (!sorted) return fail(h, BDEPTH_ERR_ARG, "-L on a file that is not coordinate-sorted names no region of the file's references: the reference's BedFilter indexes an empty region list (filtering.d:128)");
-        *count = 0; h->st = bdepth_stats{}; return 0;                                     // getReadsOverlapping([]): an empty stream
+        *empty = true; return 0;                                                          // getReadsOverlapping([]): an empty stream
     }
     if (vs.region_mode == VIEW_POSITIONAL || (vs.region_mode == VIEW_MERGED && sorted))
         if (!h->has_index) return fail(h, BDEPTH_ERR_NOINDEX, "BAM index file (.bai) must be provided");      // randomaccessmanager.d:197-202
     // per-reference slices: starts and ends each sorted (BED: merged as parseBed merges, touching regions included, bed.d:43-58)
-    std::vector<bdepth_region> plan;
+    plan.clear();
     if (vs.region_mode != VIEW_ALL) {
         std::vector<uint32_t> off(nref + 1, 0), S, E;
         if (vs.region_mode == VIEW_MERGED) {
@@ -2087,12 +2189,90 @@ int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* o, uint64_t* coun
         vs.fprog = h->vc_prog.as<FilterProg>();
     }
     h->vsel = vs;
+    return 0;
+}
+
+// ---- view -c ----------------------------------------------------------------------------------------------------------------------
+// ReadCounter over view_main's selection (sambamba/view.d:265-368): K1 + K2 as in every run, then k_view_count per sub-batch.  Regions on a
+// coordinate-sorted file with a usable index stage only their BAI chunks (plan_sparse, with the view's regions in place of the handle's for the
+// duration of the run); otherwise every record of the file is scanned.  The handle's depth settings are not used and stay as they were.
+int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* o, uint64_t* count) {
+    if (!h) return BDEPTH_ERR_ARG;
+    if (!o || !count || (o->n_regions && !o->regions)) return fail(h, BDEPTH_ERR_ARG, "null argument");
+    if (o->regions_from < BDEPTH_VIEW_ALL || o->regions_from > BDEPTH_VIEW_POSITIONAL) return fail(h, BDEPTH_ERR_ARG, "regions_from: %d", o->regions_from);
+    if (!h->extra.empty()) return fail(h, BDEPTH_ERR_ARG, "view reads one BAM file: this handle has several inputs (bdepth_add_input)");
+    std::vector<bdepth_region> plan; bool empty = false;
+    int rc = view_setup(h, o, o->regions, o->n_regions, o->n_unmapped, plan, &empty); if (rc) return rc;
+    if (empty) { *count = 0; h->st = bdepth_stats{}; return 0; }
     std::swap(h->regions, plan);
-    const int rc = run_pipeline(h, RUN_VIEW_COUNT, nullptr);
+    rc = run_pipeline(h, RUN_VIEW_COUNT, nullptr);
     std::swap(h->regions, plan);
     if (rc) return rc;
     *count = h->vc_host[0];
     h->st.ms_total_device = h->st.ms_h2d + h->st.ms_inflate + h->st.ms_scan + h->st.ms_coverage + h->st.ms_reduce;
+    return 0;
+}
+
+// ---- view (SAM text) -------------------------------------------------------------------------------------------------------------
+// SamSerializer over view_main's reads (utils/view/alignmentrangeprocessor.d:97-106): the same selection as view -c, and the lines are written
+// inside the pipeline, sub-batch by sub-batch (view_text_sub).  Positional regions are joined as the reference joins them (view.d:308-366): one
+// pipeline run per region argument, in the order given, each staging only that region's BAI chunks ('*' scans the whole file).
+int bdepth_run_view_text(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb cb, void* user) {
+    if (!h) return BDEPTH_ERR_ARG;
+    if (!o || (o->n_regions && !o->regions)) return fail(h, BDEPTH_ERR_ARG, "null argument");
+    if (o->regions_from < BDEPTH_VIEW_ALL || o->regions_from > BDEPTH_VIEW_POSITIONAL) return fail(h, BDEPTH_ERR_ARG, "regions_from: %d", o->regions_from);
+    if (!h->extra.empty()) return fail(h, BDEPTH_ERR_ARG, "view reads one BAM file: this handle has several inputs (bdepth_add_input)");
+    if (o->n_unmapped) return fail(h, BDEPTH_ERR_ARG, "n_unmapped: give each '*' in its place in the region list (ref_id BDEPTH_VIEW_UNMAPPED)");
+    const bool positional = o->regions_from == BDEPTH_VIEW_POSITIONAL;
+    if (positional && h->world > 1) return fail(h, BDEPTH_ERR_ARG, "positional regions on several ranks: each region's lines would be split over the ranks (run them on one GPU)");
+    const size_t nref = h->hdr.ref_len.size();
+    int rc = init_device(h); if (rc) return rc;
+    auto& V = h->vt;
+    {   // the reference names, once per call: offsets, then the names
+        std::vector<uint32_t> noff(nref + 1, 0); std::string all;
+        for (size_t r = 0; r < nref; r++) { noff[r] = (uint32_t)all.size(); all += h->hdr.ref_names[r]; }
+        noff[nref] = (uint32_t)all.size();
+        CK(V.names.ensure((nref + 1) * 4 + all.size() + 16));
+        CK(cudaMemcpy(V.names.p, noff.data(), (nref + 1) * 4, cudaMemcpyHostToDevice));
+        if (!all.empty()) CK(cudaMemcpy(V.names.as<uint8_t>() + (nref + 1) * 4, all.data(), all.size(), cudaMemcpyHostToDevice));
+        V.tab = SamTab{(const char*)(V.names.as<uint8_t>() + (nref + 1) * 4), V.names.as<uint32_t>(), (int32_t)nref, nullptr};
+    }
+    V.cb = cb; V.user = user; V.pend[0] = V.pend[1] = false; V.next = 0;
+    auto one_run = [&](const bdepth_region* regs, size_t n, uint32_t n_star, bdepth_stats& acc) -> int {
+        std::vector<bdepth_region> plan; bool empty = false;
+        int r = view_setup(h, o, regs, n, n_star, plan, &empty); if (r) return r;
+        if (empty) { h->st = bdepth_stats{}; return 0; }
+        std::swap(h->regions, plan);
+        r = run_pipeline(h, RUN_VIEW_TEXT, nullptr);
+        std::swap(h->regions, plan);
+        if (r) return r;
+        const bdepth_stats& s = h->st;
+        acc.file_bytes += s.file_bytes; acc.n_blocks += s.n_blocks; acc.n_records += s.n_records; acc.n_batches += s.n_batches; acc.gpu_launches += s.gpu_launches;
+        acc.ms_h2d += s.ms_h2d; acc.ms_inflate += s.ms_inflate; acc.ms_scan += s.ms_scan; acc.ms_reduce += s.ms_reduce; acc.ms_d2h += s.ms_d2h;
+        acc.ms_span_device += s.ms_span_device; acc.host_wall_ms += s.host_wall_ms;
+        return 0;
+    };
+    bdepth_stats acc{};
+    if (!positional) {
+        rc = one_run(o->regions, o->n_regions, 0, acc); if (rc) return rc;
+    } else {
+        // every argument is checked before the first line goes out, as view_main parses them all first
+        if (!o->n_regions) { rc = one_run(nullptr, 0, 0, acc); if (rc) return rc; }
+        for (size_t i = 0; i < o->n_regions; i++) {
+            const bdepth_region& g = o->regions[i];
+            if (g.ref_id == BDEPTH_VIEW_UNMAPPED) continue;
+            if (g.ref_id >= nref) return fail(h, BDEPTH_ERR_ARG, "region #%zu: reference %u out of range", i, g.ref_id);
+            if (g.start >= g.end) return fail(h, BDEPTH_ERR_ARG, "start must be less than end");
+        }
+        if (o->n_regions && !h->has_index) return fail(h, BDEPTH_ERR_NOINDEX, "BAM index file (.bai) must be provided");
+        for (size_t i = 0; i < o->n_regions; i++) {
+            const bdepth_region& g = o->regions[i];
+            rc = g.ref_id == BDEPTH_VIEW_UNMAPPED ? one_run(nullptr, 0, 1, acc) : one_run(&g, 1, 0, acc);
+            if (rc) return rc;
+        }
+    }
+    h->st = acc;
+    h->st.ms_total_device = h->st.ms_h2d + h->st.ms_inflate + h->st.ms_scan + h->st.ms_reduce + h->st.ms_d2h;
     return 0;
 }
 

@@ -1364,13 +1364,10 @@ struct ViewSel {
     uint32_t n_reg_refs;                           // references with a slice: reg_off has n_reg_refs + 1 entries
     const uint32_t* reg_off; const uint32_t* reg_s; const uint32_t* reg_e;      // regions of reference r: [reg_off[r], reg_off[r + 1]), starts and ends each sorted
 };
-__global__ void __launch_bounds__(256) k_view_count(RecordSoA soa, const uint8_t* __restrict__ u, uint32_t R, int64_t own_from, ViewSel vs, unsigned long long* __restrict__ out) {
-    __shared__ unsigned long long s_sum;
-    if (threadIdx.x == 0) s_sum = 0;
-    __syncthreads();
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+// The multiplicity of record r of a sub-batch under the selection (shared by k_view_count and the SAM text kernels k_sam_len).
+__device__ __forceinline__ unsigned long long view_select(const RecordSoA& soa, const uint8_t* __restrict__ u, uint32_t r, int64_t own_from, const ViewSel& vs) {
     unsigned long long m = 0;
-    if (r < R && soa.off[r] - 4 >= own_from) {
+    if (soa.off[r] - 4 >= own_from) {
         const int64_t o = soa.off[r];                          // refID field
         const uint32_t flag = soa.meta[r] >> 16, ncl = soa.ncl[r], l_name = ncl & 0xFFu, n_cigar = (ncl >> 8) & 0xFFFFu;
         bool keep = (flag & vs.flag_set) == vs.flag_set && (flag & vs.flag_unset) == 0;
@@ -1401,6 +1398,14 @@ __global__ void __launch_bounds__(256) k_view_count(RecordSoA soa, const uint8_t
             }
         }
     }
+    return m;
+}
+__global__ void __launch_bounds__(256) k_view_count(RecordSoA soa, const uint8_t* __restrict__ u, uint32_t R, int64_t own_from, ViewSel vs, unsigned long long* __restrict__ out) {
+    __shared__ unsigned long long s_sum;
+    if (threadIdx.x == 0) s_sum = 0;
+    __syncthreads();
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long m = r < R ? view_select(soa, u, r, own_from, vs) : 0ull;
     for (int s = 16; s; s >>= 1) m += __shfl_xor_sync(0xFFFFFFFFu, m, s);
     if ((threadIdx.x & 31) == 0 && m) atomicAdd(&s_sum, m);
     __syncthreads();
@@ -1552,6 +1557,284 @@ __global__ void __launch_bounds__(256) k_text_write_ms(TextParamsMS tp, const ui
     uint32_t woff = 0; for (uint32_t w = 0; w < warp; w++) woff += wsum[w];
     char* p = out + tile_off[blockIdx.x] + woff + (incl - mine);
     for (int k = 0; k < 4; k++) { if (!len[k]) continue; uint32_t i = base + threadIdx.x * 4 + k; text_rows_ms(tp, counts, win_len, idx0 + i, pos0 + i, p); p += len[k]; }
+}
+
+// ---- sambamba view: the SAM line of a record, BamRead.toSam (BioD/bio/std/hts/bam/read.d:695-760) plus '\n' (alignmentrangeprocessor.d:72-75).
+// A warp formats one record.  Every lane walks the record's fields in lock step and holds the same output cursor; the wide parts are shared out
+// -- the sequence (4-bit codes to "=ACMGRSVTWYHKDBN"), the qualities (+33), the CIGAR ops and the elements of B arrays (one per lane, offsets
+// from a warp prefix sum) -- and the fixed fields and the tag headers are written by lane 0.  sam_line<false> measures the line and
+// sam_line<true> writes it, so that the length pass (k_sam_len) and the write pass (k_sam_write) cannot disagree.
+// Refused, where the reference throws or indexes out of bounds: a refID or next refID outside [-1, n_ref) where a name is printed, an unknown
+// tag type or B element type (UnknownTagTypeException, tagvalue.d:567), a Z / H value without its NUL, a tag or B array that runs past the record.
+constexpr uint32_t SAM_ERR_REF = 1, SAM_ERR_MATE_REF = 2, SAM_ERR_TAG_TYPE = 3, SAM_ERR_B_TYPE = 4, SAM_ERR_NO_NUL = 5, SAM_ERR_OVERRUN = 6;
+struct SamTab {
+    const char* names; const uint32_t* name_off;   // reference names concatenated, n_ref + 1 offsets
+    int32_t n_ref;
+    unsigned long long* ctl;                        // [0] bytes of the sub-batch (k_text_scan), [1] longest line, [2] highest SAM_ERR_* met
+};
+
+// C's printf("%g", (double)f) for every float f, as glibc prints it (bio/core/utils/format.d:92-134): 6 significant digits rounded half to even on
+// the exact binary value, trailing zeros stripped, exponent form below 1e-4 and from 1e6 on with at least two exponent digits, inf / nan with
+// their sign.  f = m * 2^e exactly (m < 2^24); the digits are floor(f / 10^k) for k = X - 5 by long division of two integers of at most
+// 256 bits -- no floating-point step, so ties such as 1234565 round as the exact value says.  Writes at most 13 bytes to o, returns the length.
+struct SamBig { uint32_t w[8]; };
+__device__ __forceinline__ void big_mul(SamBig& a, uint32_t m) { unsigned long long c = 0; for (int i = 0; i < 8; i++) { c += (unsigned long long)a.w[i] * m; a.w[i] = (uint32_t)c; c >>= 32; } }
+__device__ __forceinline__ void big_shl(SamBig& d, const SamBig& a, uint32_t s) {
+    const uint32_t q = s >> 5, r = s & 31;
+    for (int i = 7; i >= 0; i--) {
+        const int j = i - (int)q;
+        const uint32_t hi = j >= 0 ? a.w[j] : 0u, lo = j >= 1 ? a.w[j - 1] : 0u;
+        d.w[i] = r ? (hi << r) | (lo >> (32 - r)) : hi;
+    }
+}
+__device__ __forceinline__ int big_cmp(const SamBig& a, const SamBig& b) { for (int i = 7; i >= 0; i--) if (a.w[i] != b.w[i]) return a.w[i] < b.w[i] ? -1 : 1; return 0; }
+__device__ __forceinline__ void big_sub(SamBig& a, const SamBig& b) { unsigned long long br = 0; for (int i = 0; i < 8; i++) { const unsigned long long t = (unsigned long long)a.w[i] - b.w[i] - br; a.w[i] = (uint32_t)t; br = (t >> 32) & 1u; } }
+__device__ __forceinline__ void big_pow10(SamBig& a, uint32_t k) { while (k >= 9) { big_mul(a, 1000000000u); k -= 9; } uint32_t p = 1; while (k--) p *= 10u; big_mul(a, p); }
+// floor(m * 2^e / 10^k) rounded half to even; *q_floor = the quotient before rounding (it tells whether k was right)
+__device__ __forceinline__ uint32_t sam_digits(uint32_t m, int e, int k, uint32_t* q_floor) {
+    SamBig num, den, t;
+    for (int i = 0; i < 8; i++) { num.w[i] = 0; den.w[i] = 0; }
+    num.w[0] = m; den.w[0] = 1;
+    if (e > 0) { big_shl(t, num, (uint32_t)e); num = t; } else if (e < 0) { big_shl(t, den, (uint32_t)-e); den = t; }
+    if (k < 0) big_pow10(num, (uint32_t)-k); else if (k > 0) big_pow10(den, (uint32_t)k);
+    uint32_t q = 0;
+    for (int b = 25; b >= 0; b--) { big_shl(t, den, (uint32_t)b); if (big_cmp(num, t) >= 0) { big_sub(num, t); q |= 1u << b; } }
+    *q_floor = q;
+    big_shl(t, num, 1);                                     // the remainder against half the divisor
+    const int c = big_cmp(t, den);
+    return q + ((c > 0 || (c == 0 && (q & 1u))) ? 1u : 0u);
+}
+__device__ __forceinline__ uint32_t sam_fmt_g(uint32_t bits, char* o) {      // bits: the float's IEEE-754 bit pattern
+    const uint32_t ex = (bits >> 23) & 0xFFu, fr = bits & 0x7FFFFFu;
+    uint32_t n = 0;
+    if (bits >> 31) o[n++] = '-';
+    if (ex == 0xFFu) { const char* s = fr ? "nan" : "inf"; o[n] = s[0]; o[n + 1] = s[1]; o[n + 2] = s[2]; return n + 3; }
+    const uint32_t m = ex ? (fr | 0x800000u) : fr;
+    if (!m) { o[n] = '0'; return n + 1; }
+    const int e = ex ? (int)ex - 150 : -149;
+    const int E = 31 - __clz((int)m) + e;                   // 2^E <= f < 2^(E+1)
+    int X = (E * 78913) >> 18;                              // floor(E * log10(2)): the decimal exponent is X or X + 1
+    uint32_t D = 0, q = 0;
+    for (;;) {
+        D = sam_digits(m, e, X - 5, &q);
+        if (q >= 1000000u) { X++; continue; }
+        if (q < 100000u) { X--; continue; }
+        break;
+    }
+    if (D == 1000000u) { D = 100000u; X++; }                 // rounding carried into a seventh digit
+    char d[6];
+    for (int i = 5; i >= 0; i--) { d[i] = (char)('0' + D % 10u); D /= 10u; }
+    if (X < -4 || X >= 6) {
+        int nd = 6; while (nd > 1 && d[nd - 1] == '0') nd--;
+        o[n++] = d[0];
+        if (nd > 1) { o[n++] = '.'; for (int i = 1; i < nd; i++) o[n++] = d[i]; }
+        o[n++] = 'e'; o[n++] = X < 0 ? '-' : '+';
+        const uint32_t ax = (uint32_t)(X < 0 ? -X : X);
+        o[n++] = (char)('0' + ax / 10u); o[n++] = (char)('0' + ax % 10u);
+        return n;
+    }
+    int nd = 6; while (nd > X + 1 && nd > 0 && d[nd - 1] == '0') nd--;      // digits after the integer part that stay
+    if (X >= 0) {
+        for (int i = 0; i <= X; i++) o[n++] = d[i];
+        if (nd > X + 1) { o[n++] = '.'; for (int i = X + 1; i < nd; i++) o[n++] = d[i]; }
+    } else {
+        o[n++] = '0'; o[n++] = '.';
+        for (int i = 0; i < -X - 1; i++) o[n++] = '0';
+        for (int i = 0; i < nd; i++) o[n++] = d[i];
+    }
+    return n;
+}
+
+__device__ __forceinline__ uint32_t sam_warp_incl(uint32_t v, uint32_t lane) {
+    for (int s = 1; s < 32; s <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, v, s); if (lane >= (uint32_t)s) v += t; }
+    return v;
+}
+__device__ __forceinline__ uint32_t dec_len_i(int64_t v) { return v < 0 ? 1u + dec_digits((uint32_t)(-v)) : dec_digits((uint32_t)v); }
+__device__ __forceinline__ char* put_dec_i(char* p, int64_t v) { if (v < 0) { *p++ = '-'; v = -v; } return put_dec(p, (uint32_t)v); }
+// a B array element or an integer tag value of BAM type t at p
+__device__ __forceinline__ int64_t sam_int(uint8_t t, const uint8_t* p) {
+    switch (t) {
+        case 'c': return (int8_t)p[0];
+        case 'C': return p[0];
+        case 's': return (int16_t)(p[0] | (p[1] << 8));
+        case 'S': return (uint16_t)(p[0] | (p[1] << 8));
+        case 'i': return (int32_t)ldu32(p);
+        default: return ldu32(p);                            // 'I'
+    }
+}
+__device__ __forceinline__ uint32_t sam_int_size(uint8_t t) { return (t == 'c' || t == 'C') ? 1u : (t == 's' || t == 'S') ? 2u : (t == 'i' || t == 'I' || t == 'f') ? 4u : 0u; }
+
+template <bool WRITE>
+__device__ uint32_t sam_line(const uint8_t* __restrict__ p, const SamTab& t, char* __restrict__ out, uint32_t lane) {
+    // p: the record's refID field; the record is the block_size bytes from there
+    const uint32_t bs = ldu32(p - 4);
+    const int32_t ref = (int32_t)ldu32(p), pos = (int32_t)ldu32(p + 4), l_seq = (int32_t)ldu32(p + 16), nref = (int32_t)ldu32(p + 20), npos = (int32_t)ldu32(p + 24), tlen = (int32_t)ldu32(p + 28);
+    const uint32_t bmn = ldu32(p + 8), fnc = ldu32(p + 12), l_name = bmn & 0xFFu, mapq = (bmn >> 8) & 0xFFu, flag = fnc >> 16, n_cig = fnc & 0xFFFFu;
+    const bool w0 = WRITE && lane == 0;
+    uint32_t err = 0;
+    if (ref < -1 || ref >= t.n_ref) err = SAM_ERR_REF;
+    else if (nref != ref && (nref < -1 || nref >= t.n_ref)) err = SAM_ERR_MATE_REF;
+    const uint64_t a0 = 32ull + l_name + 4ull * n_cig + ((uint64_t)(uint32_t)l_seq + 1) / 2 + (uint32_t)l_seq;
+    if (!err && (l_seq < 0 || a0 > bs)) err = SAM_ERR_OVERRUN;
+    if (err) { if (lane == 0) atomicMax(&t.ctl[2], (unsigned long long)err); return 0; }
+    uint32_t at = 0;
+    // QNAME FLAG RNAME POS MAPQ
+    const uint32_t nq = l_name ? l_name - 1 : 0;
+    if (WRITE) for (uint32_t i = lane; i < nq; i += 32) out[i] = (char)p[32 + i];
+    at = nq;
+    if (w0) { char* q = out + at; *q++ = '\t'; put_dec(q, flag); }
+    at += 1 + dec_digits(flag) + 1;
+    if (w0) out[at - 1] = '\t';
+    if (ref == -1) { if (w0) out[at] = '*'; at++; }
+    else { const uint32_t a = t.name_off[ref], n = t.name_off[ref + 1] - a; if (WRITE) for (uint32_t i = lane; i < n; i += 32) out[at + i] = t.names[a + i]; at += n; }
+    const int32_t pos1 = (int32_t)((uint32_t)pos + 1u), npos1 = (int32_t)((uint32_t)npos + 1u);      // D's int arithmetic wraps
+    if (w0) { char* q = out + at; *q++ = '\t'; q = put_dec_i(q, pos1); *q++ = '\t'; q = put_dec(q, mapq); *q = '\t'; }
+    at += 1 + dec_len_i(pos1) + 1 + dec_digits(mapq) + 1;
+    // CIGAR: one op per lane, "MIDNSHP=X" and '?' beyond (cigar.d:107-111,138-143)
+    const uint8_t* cg = p + 32 + l_name;
+    if (!n_cig) { if (w0) out[at] = '*'; at++; }
+    for (uint32_t b0 = 0; b0 < n_cig; b0 += 32) {
+        const uint32_t i = b0 + lane; uint32_t c = 0, len = 0;
+        if (i < n_cig) { c = ldu32(cg + 4 * i); len = dec_digits(c >> 4) + 1; }
+        const uint32_t incl = sam_warp_incl(len, lane);
+        if (WRITE && i < n_cig) { char* q = put_dec(out + at + incl - len, c >> 4); *q = "MIDNSHP=X???????"[c & 15]; }
+        at += __shfl_sync(0xFFFFFFFFu, incl, 31);
+    }
+    // RNEXT PNEXT TLEN
+    if (w0) out[at] = '\t';
+    at++;
+    if (nref == ref || nref == -1) { if (w0) out[at] = nref == -1 ? '*' : '='; at++; }
+    else { const uint32_t a = t.name_off[nref], n = t.name_off[nref + 1] - a; if (WRITE) for (uint32_t i = lane; i < n; i += 32) out[at + i] = t.names[a + i]; at += n; }
+    if (w0) { char* q = out + at; *q++ = '\t'; q = put_dec_i(q, npos1); *q++ = '\t'; q = put_dec_i(q, tlen); *q = '\t'; }
+    at += 1 + dec_len_i(npos1) + 1 + dec_len_i(tlen) + 1;
+    // SEQ QUAL
+    const uint8_t* sq = cg + 4 * n_cig; const uint8_t* qs = sq + ((uint32_t)l_seq + 1) / 2;
+    if (!l_seq) { if (w0) out[at] = '*'; at++; }
+    else { if (WRITE) for (uint32_t i = lane; i < (uint32_t)l_seq; i += 32) { const uint8_t b = sq[i >> 1]; out[at + i] = "=ACMGRSVTWYHKDBN"[(i & 1) ? (b & 15) : (b >> 4)]; } at += (uint32_t)l_seq; }
+    if (w0) out[at] = '\t';
+    at++;
+    if (!l_seq || qs[0] == 0xFFu) { if (w0) out[at] = '*'; at++; }
+    else { if (WRITE) for (uint32_t i = lane; i < (uint32_t)l_seq; i += 32) out[at + i] = (char)(uint8_t)(qs[i] + 33u); at += (uint32_t)l_seq; }
+    // tags, in stored order, while at least 2 bytes remain (read.d:1173-1186; tagvalue.d:468-504)
+    const uint8_t* ax = p + a0; const uint32_t alen = bs - (uint32_t)a0;
+    uint32_t off = 0;
+    while (off + 1 < alen) {
+        if (off + 2 >= alen) { err = SAM_ERR_OVERRUN; break; }
+        const uint8_t ty = ax[off + 2];
+        if (w0) { out[at] = '\t'; out[at + 1] = (char)ax[off]; out[at + 2] = (char)ax[off + 1]; out[at + 3] = ':'; }
+        at += 4; off += 3;
+        if (ty == 'A') {
+            if (off + 1 > alen) { err = SAM_ERR_OVERRUN; break; }
+            if (w0) { out[at] = 'A'; out[at + 1] = ':'; out[at + 2] = (char)ax[off]; }
+            at += 3; off += 1;
+        } else if (ty == 'c' || ty == 'C' || ty == 's' || ty == 'S' || ty == 'i' || ty == 'I') {
+            const uint32_t sz = sam_int_size(ty);
+            if (off + sz > alen) { err = SAM_ERR_OVERRUN; break; }
+            const int64_t v = sam_int(ty, ax + off);
+            if (w0) { out[at] = 'i'; out[at + 1] = ':'; put_dec_i(out + at + 2, v); }
+            at += 2 + dec_len_i(v); off += sz;
+        } else if (ty == 'f') {
+            if (off + 4 > alen) { err = SAM_ERR_OVERRUN; break; }
+            char g[16]; const uint32_t n = sam_fmt_g(ldu32(ax + off), g);
+            if (w0) { out[at] = 'f'; out[at + 1] = ':'; for (uint32_t i = 0; i < n; i++) out[at + 2 + i] = g[i]; }
+            at += 2 + n; off += 4;
+        } else if (ty == 'Z' || ty == 'H') {
+            uint32_t nul = alen;                                // the warp looks for the NUL 32 bytes at a time
+            for (uint32_t b0 = off; b0 < alen; b0 += 32) {
+                const uint32_t i = b0 + lane;
+                const unsigned z = __ballot_sync(0xFFFFFFFFu, i < alen && ax[i] == 0);
+                if (z) { nul = b0 + (uint32_t)__ffs((int)z) - 1; break; }
+            }
+            if (nul == alen) { err = SAM_ERR_NO_NUL; break; }
+            if (w0) { out[at] = (char)ty; out[at + 1] = ':'; }
+            if (WRITE) for (uint32_t i = lane; i < nul - off; i += 32) out[at + 2 + i] = (char)ax[off + i];
+            at += 2 + (nul - off); off = nul + 1;
+        } else if (ty == 'B') {
+            if (off + 5 > alen) { err = SAM_ERR_OVERRUN; break; }
+            const uint8_t et = ax[off]; const uint32_t n = ldu32(ax + off + 1), sz = sam_int_size(et);
+            if (!sz) { err = SAM_ERR_B_TYPE; break; }
+            off += 5;
+            if ((uint64_t)n * sz > alen - off) { err = SAM_ERR_OVERRUN; break; }
+            if (w0) { out[at] = 'B'; out[at + 1] = ':'; out[at + 2] = (char)et; out[at + 3] = ','; }
+            at += 4;
+            for (uint32_t b0 = 0; b0 < n; b0 += 32) {           // element i is preceded by ',' when i > 0
+                const uint32_t i = b0 + lane; uint32_t len = 0; char g[16]; int64_t v = 0;
+                if (i < n) {
+                    if (et == 'f') len = sam_fmt_g(ldu32(ax + off + 4 * i), g);
+                    else { v = sam_int(et, ax + off + sz * i); len = dec_len_i(v); }
+                    len += i ? 1u : 0u;
+                }
+                const uint32_t incl = sam_warp_incl(len, lane);
+                if (WRITE && i < n) {
+                    char* q = out + at + incl - len;
+                    if (i) *q++ = ',';
+                    if (et == 'f') { for (uint32_t k = 0; k < len - (i ? 1u : 0u); k++) q[k] = g[k]; }
+                    else put_dec_i(q, v);
+                }
+                at += __shfl_sync(0xFFFFFFFFu, incl, 31);
+            }
+            off += n * sz;
+        } else { err = SAM_ERR_TAG_TYPE; break; }
+    }
+    if (err) { if (lane == 0) atomicMax(&t.ctl[2], (unsigned long long)err); return 0; }
+    if (w0) out[at] = '\n';
+    return at + 1;
+}
+
+// pass 1: len[r] = bytes of record r's line (0: not selected), warp per record; the longest line into ctl[1]
+__global__ void __launch_bounds__(256, 1) k_sam_len(RecordSoA soa, const uint8_t* __restrict__ u, uint32_t R, int64_t own_from, ViewSel vs, SamTab t, uint32_t* __restrict__ len) {
+    const uint32_t lane = threadIdx.x & 31, nw = gridDim.x * (blockDim.x >> 5);
+    uint32_t mx = 0;
+    for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < R; r += nw) {
+        uint32_t n = 0;
+        if (view_select(soa, u, r, own_from, vs)) n = sam_line<false>(u + soa.off[r], t, nullptr, lane);
+        if (lane == 0) len[r] = n;
+        mx = n > mx ? n : mx;
+    }
+    if (lane == 0 && mx) atomicMax(&t.ctl[1], (unsigned long long)mx);
+}
+// device-wide exclusive scan of len[0, R) into 64-bit offsets: tile sums (SAM_SCAN_TILE records per CTA), k_text_scan over the tiles, then
+// each tile scans its records from its tile offset
+constexpr uint32_t SAM_SCAN_TILE = 2048;
+__global__ void __launch_bounds__(256) k_sam_tile_sum(const uint32_t* __restrict__ len, uint32_t R, uint32_t* __restrict__ tile_sum) {
+    __shared__ uint32_t wsum[8];
+    const uint32_t base = blockIdx.x * SAM_SCAN_TILE + threadIdx.x * 8;
+    uint32_t s = 0;
+    for (uint32_t k = 0; k < 8; k++) if (base + k < R) s += len[base + k];
+    for (int sh = 16; sh; sh >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, sh);
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) { uint32_t a = 0; for (int w = 0; w < 8; w++) a += wsum[w]; tile_sum[blockIdx.x] = a; }
+}
+__global__ void __launch_bounds__(256) k_sam_scan_apply(const uint32_t* __restrict__ len, uint32_t R, const unsigned long long* __restrict__ tile_off, unsigned long long* __restrict__ off) {
+    __shared__ uint32_t wsum[8];
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, base = blockIdx.x * SAM_SCAN_TILE + threadIdx.x * 8;
+    uint32_t v[8], mine = 0;
+    for (uint32_t k = 0; k < 8; k++) { v[k] = base + k < R ? len[base + k] : 0u; mine += v[k]; }
+    const uint32_t incl = sam_warp_incl(mine, lane);
+    if (lane == 31) wsum[warp] = incl;
+    __syncthreads();
+    uint32_t woff = 0; for (uint32_t w = 0; w < warp; w++) woff += wsum[w];
+    unsigned long long a = tile_off[blockIdx.x] + woff + (incl - mine);
+    for (uint32_t k = 0; k < 8; k++) if (base + k < R) { off[base + k] = a; a += v[k]; }
+}
+// piece cuts: cut_r[j] = the first record whose line starts at or after j * piece (R past the end), cut_o[j] its offset (the total past the end)
+__global__ void k_sam_cut(const unsigned long long* __restrict__ off, uint32_t R, unsigned long long total, unsigned long long piece, uint32_t n_cuts,
+                          uint32_t* __restrict__ cut_r, unsigned long long* __restrict__ cut_o) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n_cuts; j += gridDim.x * blockDim.x) {
+        const unsigned long long target = (unsigned long long)j * piece;
+        uint32_t a = 0, b = R;
+        while (a < b) { const uint32_t mid = (a + b) >> 1; if (off[mid] < target) a = mid + 1; else b = mid; }
+        cut_r[j] = a; cut_o[j] = a < R ? off[a] : total;
+    }
+}
+// pass 2: the lines of records [r0, r1) into out, at their offsets relative to off[r0]; warp per record
+__global__ void __launch_bounds__(256, 1) k_sam_write(const int64_t* __restrict__ rec_off, const uint8_t* __restrict__ u, uint32_t r0, uint32_t r1, const uint32_t* __restrict__ len,
+                                                   const unsigned long long* __restrict__ off, SamTab t, char* __restrict__ out) {
+    const uint32_t lane = threadIdx.x & 31, nw = gridDim.x * (blockDim.x >> 5);
+    const unsigned long long base = off[r0];
+    for (uint32_t r = r0 + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5); r < r1; r += nw)
+        if (len[r]) sam_line<true>(u + rec_off[r], t, out + (off[r] - base), lane);
 }
 
 }  // namespace bdk

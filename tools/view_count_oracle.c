@@ -1,4 +1,5 @@
-/* view_count_oracle.c -- CPU restatement of `sambamba view -c` (TEST INFRASTRUCTURE: the checker the GPU count is compared with).
+/* view_count_oracle.c -- CPU restatement of `sambamba view -c` and of `sambamba view`'s SAM lines (TEST INFRASTRUCTURE: the checker the GPU
+ * count and text are compared with).
  *
  * What is restated (sambamba/view.d:265-379), record by record, without shortcuts:
  *   - FlagBitFilter (utils/common/filtering.d:176-187) and SubsampleFilter (:340-371, FNV-1a 64 over the name, then the seed's 8 bytes);
@@ -12,9 +13,15 @@
  * the state machine selects the same reads from either, and this file does not depend on the engine's index code.  -F is not restated here:
  * the tests apply a Python statement of the query and count the reduced file.
  *
- * Library: view_count_oracle(), view_count_oracle_hash(), view_count_oracle_error().  With -DORACLE_MAIN also a CLI:
- *   view_count_oracle view -c [--num-filter=I1/I2] [-s FRAC] [--subsampling-seed=SEED] [-L BED] in.bam [region ...]
- * which prints the count as `sambamba view -c` does, or "sambamba-view: <msg>" and exit code 1 for the errors it restates. */
+ * The SAM line of a selected read is a literal C statement of BamRead.toSam (BioD/bio/std/hts/bam/read.d:695-760) plus '\n'
+ * (alignmentrangeprocessor.d:72-75), with the tag values of tagvalue.d:468-504 and floats through snprintf("%g", (double)f) as
+ * bio/core/utils/format.d:92-134 does.  Where the reference throws or indexes out of bounds (an unknown tag type, a tag running past the record,
+ * a Z / H value without its NUL, a reference ID outside [-1, n_ref) that is printed), the text entry point returns an error.
+ * Library: view_count_oracle(), view_text_oracle(), view_text_oracle_free(), view_count_oracle_hash(), view_count_oracle_error().  With
+ * -DORACLE_MAIN also a CLI:
+ *   view_count_oracle view [-c] [--num-filter=I1/I2] [-s FRAC] [--subsampling-seed=SEED] [-L BED] in.bam [region ...]
+ * which prints the count as `sambamba view -c` does, or without -c the SAM lines (no header), or "sambamba-view: <msg>" and exit code 1 for the
+ * errors it restates. */
 #include <ctype.h>
 #include <errno.h>
 #include <math.h>
@@ -27,7 +34,7 @@
 static char g_err[512];
 const char* view_count_oracle_error(void) { return g_err; }
 
-typedef struct { int32_t ref, pos; uint16_t flag; int64_t bc; const uint8_t* name; uint32_t l_name; } Rec;
+typedef struct { int32_t ref, pos; uint16_t flag; int64_t bc; const uint8_t* name; uint32_t l_name; const uint8_t* p; uint32_t bs; } Rec;      /* p: the refID field, bs: block_size */
 typedef struct { uint8_t* u; size_t n; int n_ref; char** names; int sorted; Rec* r; size_t nr; } Bam;
 
 static uint32_t rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
@@ -76,7 +83,7 @@ static int bam_load(const char* path, Bam* b) {
         Rec* x = &b->r[b->nr++];
         x->ref = (int32_t)rd32(p); x->pos = (int32_t)rd32(p + 4);
         uint32_t bmn = rd32(p + 8), fnc = rd32(p + 12);
-        x->l_name = bmn & 0xFF; x->flag = (uint16_t)(fnc >> 16);
+        x->l_name = bmn & 0xFF; x->flag = (uint16_t)(fnc >> 16); x->p = p; x->bs = bs;
         uint32_t nc = fnc & 0xFFFF; x->name = p + 32;
         x->bc = 0;
         if (!(x->flag & 4)) for (uint32_t k = 0; k < nc; k++) { uint32_t c = rd32(p + 32 + x->l_name + 4 * k), op = c & 15; if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) x->bc += c >> 4; }      /* basesCovered, read.d:255-262 */
@@ -95,14 +102,101 @@ uint64_t view_count_oracle_hash(const uint8_t* name, size_t len, uint64_t seed) 
 
 typedef struct { uint32_t ref, start, end; } Reg;
 
+/* Where selected reads go: counted, or formatted as SAM lines into a growing buffer. */
+typedef struct { int text; uint64_t cnt; char* buf; size_t len, cap; int err; } Out;
+static void out_put(Out* o, const void* s, size_t n) {
+    if (o->len + n > o->cap) { o->cap = (o->len + n) * 2 + 4096; o->buf = realloc(o->buf, o->cap); }
+    memcpy(o->buf + o->len, s, n); o->len += n;
+}
+static void out_str(Out* o, const char* s) { out_put(o, s, strlen(s)); }
+static void out_fmt(Out* o, const char* fmt, long long v) { char t[32]; int n = snprintf(t, sizeof t, fmt, v); out_put(o, t, (size_t)n); }
+static void out_g(Out* o, float f) { char t[64]; int n = snprintf(t, sizeof t, "%g", (double)f); out_put(o, t, (size_t)n); }
+static uint32_t val_size(uint8_t t) { return (t == 'c' || t == 'C') ? 1 : (t == 's' || t == 'S') ? 2 : (t == 'i' || t == 'I' || t == 'f') ? 4 : 0; }
+static void out_val(Out* o, uint8_t t, const uint8_t* e) {                /* one integer (signed or unsigned as stored) or float value */
+    switch (t) {
+        case 'c': out_fmt(o, "%lld", (int8_t)e[0]); break;
+        case 'C': out_fmt(o, "%lld", e[0]); break;
+        case 's': out_fmt(o, "%lld", (int16_t)(e[0] | (e[1] << 8))); break;
+        case 'S': out_fmt(o, "%lld", (uint16_t)(e[0] | (e[1] << 8))); break;
+        case 'i': out_fmt(o, "%lld", (int32_t)rd32(e)); break;
+        case 'I': out_fmt(o, "%lld", rd32(e)); break;
+        default: { uint32_t w = rd32(e); float f; memcpy(&f, &w, 4); out_g(o, f); }
+    }
+}
+static int sam_fail(Out* o, const char* m) { if (!o->err) snprintf(g_err, sizeof g_err, "%s", m); o->err = 1; return -1; }
+/* BamRead.toSam (read.d:695-760) of one record, '\n' after it */
+static int sam_line(const Bam* b, const Rec* x, Out* o) {
+    const uint8_t* p = x->p; const uint32_t bs = x->bs;
+    const int32_t ref = (int32_t)rd32(p), pos = (int32_t)rd32(p + 4), l_seq = (int32_t)rd32(p + 16), nref = (int32_t)rd32(p + 20), npos = (int32_t)rd32(p + 24), tlen = (int32_t)rd32(p + 28);
+    const uint32_t bmn = rd32(p + 8), fnc = rd32(p + 12), l_name = bmn & 0xFF, mapq = (bmn >> 8) & 0xFF, flag = fnc >> 16, n_cig = fnc & 0xFFFF;
+    if (ref < -1 || ref >= b->n_ref) return sam_fail(o, "reference ID out of range");
+    if (nref != ref && (nref < -1 || nref >= b->n_ref)) return sam_fail(o, "mate reference ID out of range");
+    const uint64_t a0 = 32ull + l_name + 4ull * n_cig + ((uint64_t)(uint32_t)l_seq + 1) / 2 + (uint32_t)l_seq;
+    if (l_seq < 0 || a0 > bs) return sam_fail(o, "record fields run past block_size");
+    out_put(o, p + 32, l_name ? l_name - 1 : 0);                         /* name */
+    out_fmt(o, "\t%lld\t", flag);
+    if (ref == -1) out_str(o, "*"); else out_str(o, b->names[ref]);
+    out_fmt(o, "\t%lld", (int32_t)((uint32_t)pos + 1u));                  /* position + 1 in D's int: wraps */
+    out_fmt(o, "\t%lld\t", mapq);
+    const uint8_t* cg = p + 32 + l_name;
+    if (!n_cig) out_str(o, "*");
+    for (uint32_t i = 0; i < n_cig; i++) { uint32_t c = rd32(cg + 4 * i); out_fmt(o, "%lld", c >> 4); out_put(o, &"MIDNSHP=X???????"[c & 15], 1); }
+    out_str(o, "\t");
+    if (nref == ref) out_str(o, nref == -1 ? "*\t" : "=\t");
+    else if (nref == -1) out_str(o, "*\t");
+    else { out_str(o, b->names[nref]); out_str(o, "\t"); }
+    out_fmt(o, "%lld\t", (int32_t)((uint32_t)npos + 1u));
+    out_fmt(o, "%lld\t", tlen);
+    const uint8_t* sq = cg + 4 * n_cig; const uint8_t* qs = sq + ((uint32_t)l_seq + 1) / 2;
+    if (l_seq == 0) out_str(o, "*");
+    for (int32_t i = 0; i < l_seq; i++) out_put(o, &"=ACMGRSVTWYHKDBN"[(i & 1) ? (sq[i >> 1] & 15) : (sq[i >> 1] >> 4)], 1);
+    out_str(o, "\t");
+    if (l_seq == 0 || qs[0] == 0xFF) out_str(o, "*");
+    else for (int32_t i = 0; i < l_seq; i++) { char c = (char)(uint8_t)(qs[i] + 33); out_put(o, &c, 1); }
+    const uint8_t* ax = p + a0; const size_t alen = bs - a0;
+    size_t off = 0;
+    while (off + 1 < alen) {                                                /* opApply, read.d:1173-1186 */
+        out_str(o, "\t"); out_put(o, ax + off, 2); out_str(o, ":");
+        off += 2;
+        if (off >= alen) return sam_fail(o, "tag runs past the record");
+        const uint8_t t = ax[off++];
+        const uint32_t sz = val_size(t);
+        if (t == 'A') {
+            if (off + 1 > alen) return sam_fail(o, "tag runs past the record");
+            out_str(o, "A:"); out_put(o, ax + off, 1); off += 1;
+        } else if (sz) {                                                    /* c C s S i I: "i:", f: "f:" */
+            if (off + sz > alen) return sam_fail(o, "tag runs past the record");
+            out_str(o, t == 'f' ? "f:" : "i:"); out_val(o, t, ax + off); off += sz;
+        } else if (t == 'Z' || t == 'H') {
+            const uint8_t* z = memchr(ax + off, 0, alen - off);
+            if (!z) return sam_fail(o, "Z or H value without its NUL");
+            out_put(o, &t, 1); out_str(o, ":"); out_put(o, ax + off, (size_t)(z - (ax + off))); off = (size_t)(z - ax) + 1;
+        } else if (t == 'B') {
+            if (off + 5 > alen) return sam_fail(o, "B array runs past the record");
+            const uint8_t et = ax[off]; const uint32_t n = rd32(ax + off + 1), esz = val_size(et); off += 5;
+            if (!esz) return sam_fail(o, "unknown B array element type");
+            if ((uint64_t)n * esz > alen - off) return sam_fail(o, "B array runs past the record");
+            out_str(o, "B:"); out_put(o, &et, 1); out_str(o, ",");
+            for (uint32_t i = 0; i < n; i++) { if (i) out_str(o, ","); out_val(o, et, ax + off + (size_t)esz * i); }
+            off += (size_t)n * esz;
+        } else return sam_fail(o, "unknown tag type");
+    }
+    out_str(o, "\n");
+    return 0;
+}
+static void emit(const Bam* b, const Rec* x, Out* o) {
+    if (!o->text) { o->cnt++; return; }
+    if (!o->err) sam_line(b, x, o);
+}
+
 /* BamReadFilter (randomaccessmanager.d:366-462): number of records of rec[0..n) the state machine yields for the sorted, non-overlapping regions. */
 static int keep_read(const Rec* x, unsigned fs, unsigned fu, int sub, uint64_t thr, uint64_t seed) {
     if ((x->flag & fs) != fs || (x->flag & fu)) return 0;
     if (sub && (view_count_oracle_hash(x->name, x->l_name ? x->l_name - 1 : 0, seed) & 0xFFFFFFFFull) >= thr) return 0;
     return 1;
 }
-static uint64_t read_filter_walk(const Bam* b, const Reg* regs, size_t nreg, size_t i0, unsigned fs, unsigned fu, int sub, uint64_t thr, uint64_t seed) {
-    uint64_t cnt = 0; size_t ri = 0; const uint32_t ref_id = regs[0].ref;
+static void read_filter_walk(const Bam* b, const Reg* regs, size_t nreg, size_t i0, unsigned fs, unsigned fu, int sub, uint64_t thr, uint64_t seed, Out* out) {
+    size_t ri = 0; const uint32_t ref_id = regs[0].ref;
     for (size_t i = i0; i < b->nr && ri < nreg;) {
         const Rec* x = &b->r[i];
         uint32_t cur = (uint32_t)x->ref;                          /* cast(uint)ref_id */
@@ -113,10 +207,9 @@ static uint64_t read_filter_walk(const Bam* b, const Reg* regs, size_t nreg, siz
         if ((uint32_t)x->pos > regs[ri].start) yield = 1;
         else if ((int64_t)(int32_t)x->pos + x->bc <= (int64_t)regs[ri].start) yield = 0;
         else yield = 1;
-        if (yield && keep_read(x, fs, fu, sub, thr, seed)) cnt++;
+        if (yield && keep_read(x, fs, fu, sub, thr, seed)) emit(b, x, out);
         i++;
     }
-    return cnt;
 }
 
 static int cmp_reg(const void* a, const void* b) {
@@ -127,14 +220,13 @@ static int cmp_reg(const void* a, const void* b) {
 }
 
 /* mode 0: every record; 1: -L regions (as parseBed hands them over: any order, merged here as nonOverlappingIntervals does, bed.d:43-58);
- * 2: positional regions (ref, start, end) in the given order plus n_star '*' queries.  Returns 0 or -1 (view_count_oracle_error()). */
-int view_count_oracle(const char* path, unsigned flag_set, unsigned flag_unset, int subsample, uint64_t threshold, uint64_t seed,
-                      int mode, const uint32_t* regs, size_t nreg, unsigned n_star, uint64_t* out) {
-    Bam b; g_err[0] = 0;
-    if (bam_load(path, &b)) { bam_free(&b); return -1; }
-    uint64_t cnt = 0; int rc = 0;
+ * 2: positional regions (ref, start, end) in the given order, a ref of 0xFFFFFFFF being '*' in its place, plus n_star '*' queries at the end.
+ * Returns 0 or -1 (view_count_oracle_error()). */
+static int view_stream(const Bam* b, unsigned flag_set, unsigned flag_unset, int subsample, uint64_t threshold, uint64_t seed,
+                       int mode, const uint32_t* regs, size_t nreg, unsigned n_star, Out* out) {
+    int rc = 0;
     if (mode == 0) {
-        for (size_t i = 0; i < b.nr; i++) cnt += (uint64_t)keep_read(&b.r[i], flag_set, flag_unset, subsample, threshold, seed);
+        for (size_t i = 0; i < b->nr; i++) if (keep_read(&b->r[i], flag_set, flag_unset, subsample, threshold, seed)) emit(b, &b->r[i], out);
     } else if (mode == 1) {
         Reg* r = malloc((nreg + 1) * sizeof(Reg)); size_t m = 0;
         for (size_t i = 0; i < nreg; i++) if (regs[3 * i + 1] < regs[3 * i + 2]) { r[m].ref = regs[3 * i]; r[m].start = regs[3 * i + 1]; r[m].end = regs[3 * i + 2]; m++; }
@@ -142,35 +234,66 @@ int view_count_oracle(const char* path, unsigned flag_set, unsigned flag_unset, 
         size_t k = 0;
         for (size_t i = 0; i < m; i++) { if (k && r[k - 1].ref == r[i].ref && r[k - 1].end >= r[i].start) { if (r[i].end > r[k - 1].end) r[k - 1].end = r[i].end; } else r[k++] = r[i]; }
         m = k;
-        if (b.sorted) {                                    /* getReadsOverlapping: one BamReadFilter per reference group, joined */
-            for (size_t g = 0; g < m;) { size_t e = g; while (e < m && r[e].ref == r[g].ref) e++; cnt += read_filter_walk(&b, r + g, e - g, 0, flag_set, flag_unset, subsample, threshold, seed); g = e; }
+        if (b->sorted) {                                   /* getReadsOverlapping: one BamReadFilter per reference group, joined */
+            for (size_t g = 0; g < m;) { size_t e = g; while (e < m && r[e].ref == r[g].ref) e++; read_filter_walk(b, r + g, e - g, 0, flag_set, flag_unset, subsample, threshold, seed, out); g = e; }
         } else if (!m) {
             snprintf(g_err, sizeof g_err, "-L on an unsorted file with no region on the file's references: BedFilter indexes an empty list"); rc = -1;
         } else {                                           /* BedFilter: trees_.length = bed.back.ref_id + 1 */
             const uint32_t ntrees = r[m - 1].ref + 1;
-            for (size_t i = 0; i < b.nr; i++) {
-                const Rec* x = &b.r[i];
+            for (size_t i = 0; i < b->nr; i++) {
+                const Rec* x = &b->r[i];
                 if (x->ref < 0 || (uint32_t)x->ref >= ntrees || !keep_read(x, flag_set, flag_unset, subsample, threshold, seed)) continue;
                 const uint32_t s = (uint32_t)x->pos, t = (uint32_t)((int32_t)x->pos + (int32_t)x->bc);
-                for (size_t j = 0; j < m; j++) if (r[j].ref == (uint32_t)x->ref && r[j].end > s && r[j].start < t) { cnt++; break; }
+                for (size_t j = 0; j < m; j++) if (r[j].ref == (uint32_t)x->ref && r[j].end > s && r[j].start < t) { emit(b, x, out); break; }
             }
         }
         free(r);
     } else {
-        for (size_t i = 0; i < nreg; i++) {
+        for (size_t i = 0; i < nreg && !rc; i++) {
             Reg one = {regs[3 * i], regs[3 * i + 1], regs[3 * i + 2]};
-            if (!(one.start < one.end)) { snprintf(g_err, sizeof g_err, "start must be less than end"); rc = -1; break; }
-            cnt += read_filter_walk(&b, &one, 1, 0, flag_set, flag_unset, subsample, threshold, seed);
+            if (one.ref == 0xFFFFFFFFu) continue;
+            if (!(one.start < one.end)) { snprintf(g_err, sizeof g_err, "start must be less than end"); rc = -1; }
+        }
+        for (size_t i = 0; i < nreg && !rc; i++) {
+            Reg one = {regs[3 * i], regs[3 * i + 1], regs[3 * i + 2]};
+            if (one.ref != 0xFFFFFFFFu) { read_filter_walk(b, &one, 1, 0, flag_set, flag_unset, subsample, threshold, seed, out); continue; }
+            /* '*' in its place: unmappedReads, the first refID -1 record, then everything to EOF */
+            size_t k = 0; while (k < b->nr && b->r[k].ref != -1) k++;
+            for (; k < b->nr; k++) if (keep_read(&b->r[k], flag_set, flag_unset, subsample, threshold, seed)) emit(b, &b->r[k], out);
         }
         for (unsigned k = 0; k < n_star && !rc; k++) {     /* unmappedReads: the first refID -1 record, then everything to EOF */
-            size_t i = 0; while (i < b.nr && b.r[i].ref != -1) i++;
-            for (; i < b.nr; i++) cnt += (uint64_t)keep_read(&b.r[i], flag_set, flag_unset, subsample, threshold, seed);
+            size_t i = 0; while (i < b->nr && b->r[i].ref != -1) i++;
+            for (; i < b->nr; i++) if (keep_read(&b->r[i], flag_set, flag_unset, subsample, threshold, seed)) emit(b, &b->r[i], out);
         }
     }
-    bam_free(&b);
-    if (!rc) *out = cnt;
+    if (!rc && out->err) rc = -1;
     return rc;
 }
+
+int view_count_oracle(const char* path, unsigned flag_set, unsigned flag_unset, int subsample, uint64_t threshold, uint64_t seed,
+                      int mode, const uint32_t* regs, size_t nreg, unsigned n_star, uint64_t* out) {
+    Bam b; g_err[0] = 0;
+    if (bam_load(path, &b)) { bam_free(&b); return -1; }
+    Out o = {0};
+    const int rc = view_stream(&b, flag_set, flag_unset, subsample, threshold, seed, mode, regs, nreg, n_star, &o);
+    bam_free(&b);
+    if (!rc) *out = o.cnt;
+    return rc;
+}
+
+/* The SAM lines `sambamba view` prints after the header, in the order of its joined stream; *text is freed with view_text_oracle_free(). */
+int view_text_oracle(const char* path, unsigned flag_set, unsigned flag_unset, int subsample, uint64_t threshold, uint64_t seed,
+                     int mode, const uint32_t* regs, size_t nreg, char** text, size_t* len) {
+    Bam b; g_err[0] = 0;
+    if (bam_load(path, &b)) { bam_free(&b); return -1; }
+    Out o = {0}; o.text = 1;
+    const int rc = view_stream(&b, flag_set, flag_unset, subsample, threshold, seed, mode, regs, nreg, 0, &o);
+    bam_free(&b);
+    if (rc) { free(o.buf); return -1; }
+    *text = o.buf; *len = o.len;
+    return 0;
+}
+void view_text_oracle_free(char* text) { free(text); }
 
 #ifdef ORACLE_MAIN
 static int die(const char* m) { fprintf(stderr, "sambamba-view: %s\n", m); return 1; }
@@ -202,7 +325,7 @@ static void parse_region(const char* s, char* ref, size_t cap, uint32_t* beg, ui
     if (q < n && s[q] == '-') { q++; v = 0; while (q < n) { if (s[q] != ',') v = v * 10 + (s[q] - '0'); q++; } *end = (uint32_t)v; }
 }
 int main(int argc, char** argv) {
-    if (argc < 2 || strcmp(argv[1], "view")) { fprintf(stderr, "usage: view_count_oracle view -c [options] in.bam [region ...]\n"); return 1; }
+    if (argc < 2 || strcmp(argv[1], "view")) { fprintf(stderr, "usage: view_count_oracle view [-c] [options] in.bam [region ...]\n"); return 1; }
     unsigned long long fs = 0, fu = 0, seed = 0; double frac = NAN; const char* bed = NULL; int count = 0;
     const char* pos_args[4096]; int npos = 0;
     for (int i = 2; i < argc; i++) {
@@ -218,7 +341,7 @@ int main(int argc, char** argv) {
         else if (!strcmp(a, "-L") && i + 1 < argc) bed = argv[++i];
         else if (npos < 4096) pos_args[npos++] = a;
     }
-    if (!count || npos < 1) { fprintf(stderr, "usage: view_count_oracle view -c [options] in.bam [region ...]\n"); return 1; }
+    if (npos < 1) { fprintf(stderr, "usage: view_count_oracle view [-c] [options] in.bam [region ...]\n"); return 1; }
     int sub = !isnan(frac); uint64_t thr = 0;
     if (sub) { double t = 4294967296.0 * frac; if (!(t >= 0)) return die("Conversion negative overflow"); if (t > 18446744073709551616.0) return die("Conversion positive overflow"); thr = t >= 18446744073709551616.0 ? UINT64_MAX : (uint64_t)t; }
     if (bed && npos > 1) return die("specifying both region and BED filename is disallowed");
@@ -247,7 +370,11 @@ int main(int argc, char** argv) {
     } else if (npos > 1) {
         mode = 2;
         for (int i = 1; i < npos; i++) {
-            if (!strcmp(pos_args[i], "*")) { n_star++; continue; }
+            if (!strcmp(pos_args[i], "*")) {               /* counted at the end; the text keeps it in its place */
+                if (count) { n_star++; continue; }
+                if (n == cap) { cap *= 2; regs = realloc(regs, cap * 3 * sizeof(uint32_t)); }
+                regs[3 * n] = 0xFFFFFFFFu; regs[3 * n + 1] = 0; regs[3 * n + 2] = 0; n++; continue;
+            }
             char ref[4096]; uint32_t beg, end; parse_region(pos_args[i], ref, sizeof ref, &beg, &end);
             int id = -1; for (int r = 0; r < b.n_ref; r++) if (!strcmp(b.names[r], ref)) id = r;
             if (id < 0) { char msg[4200]; snprintf(msg, sizeof msg, "Reference with name %s does not exist", ref); bam_free(&b); return die(msg); }
@@ -262,6 +389,13 @@ int main(int argc, char** argv) {
         }
     }
     bam_free(&b);
+    if (!count) {
+        if (mode == 2 && !n) mode = 0;
+        char* text = NULL; size_t len = 0;
+        if (view_text_oracle(pos_args[0], (unsigned)fs, (unsigned)fu, sub, thr, seed, mode, regs, n, &text, &len)) { free(regs); return die(g_err); }
+        fwrite(text, 1, len, stdout); free(text); free(regs);
+        return 0;
+    }
     uint64_t cnt = 0;
     if (view_count_oracle(pos_args[0], (unsigned)fs, (unsigned)fu, sub, thr, seed, mode, regs, n, n_star, &cnt)) { free(regs); return die(g_err); }
     free(regs);
