@@ -47,6 +47,9 @@ struct DevBuf {
     template <class T> T* as() const { return (T*)p; }
 };
 
+__global__ void k_copy_words(uint32_t* __restrict__ dst, const uint32_t* __restrict__ src, size_t n) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) dst[i] = src[i];
+}
 // Small control-plane transfers (block tables up, chain/scan results down) do not go through the copy engines:
 // those queue in order behind the bulk H2D of the compressed file and the bulk D2H of finished counters, which
 // cost every sub-batch milliseconds.  They live in mapped pinned memory and a tiny kernel moves the words.
@@ -65,10 +68,21 @@ struct HostScratch {
     uint8_t* take(size_t n) { size_t a = (used + 15) & ~size_t(15); if (a + n > cap) return nullptr; used = a + n; return hp + a; }
     uint8_t* dev(const void* host) const { return dp + ((const uint8_t*)host - hp); }
     void release() { if (hp) cudaFreeHost(hp); hp = nullptr; dp = nullptr; cap = used = 0; }
+    // up(): host words -> device buffer; down(): device words -> this scratch, readable on the host after the next synchronisation of
+    // stream s.  Both are stream-ordered kernels on s, each counted in *launches; false / nullptr: the scratch is exhausted.
+    bool up(cudaStream_t s, uint32_t* launches, void* dst_dev, const void* src, size_t bytes) {
+        if (!bytes) return true;
+        uint8_t* m = take(bytes); if (!m) return false;
+        memcpy(m, src, bytes); copy_words(s, launches, dst_dev, dev(m), bytes); return true;
+    }
+    uint8_t* down(cudaStream_t s, uint32_t* launches, const void* src_dev, size_t bytes) {
+        uint8_t* m = take(bytes ? bytes : 4); if (m && bytes) copy_words(s, launches, dev(m), src_dev, bytes);
+        return m;
+    }
+    static void copy_words(cudaStream_t s, uint32_t* launches, void* dst, const void* src, size_t bytes) {
+        BD_LAUNCH((unsigned)std::min<size_t>((bytes / 4 + 255) / 256, 512), 256, 0, s, k_copy_words)((uint32_t*)dst, (const uint32_t*)src, bytes / 4); ++*launches;
+    }
 };
-__global__ void k_copy_words(uint32_t* __restrict__ dst, const uint32_t* __restrict__ src, size_t n) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) dst[i] = src[i];
-}
 
 #ifdef BDEPTH_EMULATE_SHIM
 constexpr unsigned COUNT_GRID = 4;           // grid-stride reducer: any grid gives the same sum; the CPU emulation runs blocks one by one
@@ -81,7 +95,27 @@ constexpr uint32_t SHARD_EXTRA_BLOCKS = 8;
 constexpr uint32_t MATE_ZONE_BLOCKS = 64;       // -m on several ranks: blocks read behind the shard so that pairs cut by the boundary are seen whole
 
 enum RunMode { RUN_FULL = 0, RUN_INFLATE_ONLY = 1, RUN_SCAN_ONLY = 2, RUN_INDEX = 3, RUN_FLAGSTAT = 4, RUN_VIEW_COUNT = 5, RUN_VIEW_TEXT = 6 };
+// Several ranks with NCCL: the collective of the current run that a rank owes its peers next.  A rank that stops with an error joins it with
+// a "failed" mark (abort_collectives), so that the others stop too instead of waiting for it.
+// BOUNDARY_TABLE: depth's all-gather in exchange_boundaries; SPARSE_DECISION: a sparse region query's all-reduce that tells whether every rank's
+// chunks ended where the index says; FLAGSTAT_SUM / VIEW_SUM: the all-reduce of flagstat's counters / view's count, with the failure word.
+enum class Owed { NOTHING, BOUNDARY_TABLE, SPARSE_DECISION, FLAGSTAT_SUM, VIEW_SUM };
+// What each run mode asks of the pipeline's shared front end; per-run conditions (-m, sparse staging, ranks) are combined with it where used.
+// sub_batched: a batch is handed on chunk by chunk as K1 finishes (not with -m); may_stage_sparse: a region query stages only its regions' BAI
+// chunks (plan_sparse); loads_fprog: the depth -F program sets K2's pass bit; rewrites_lead_n: CIGARs that begin with N are rewritten to what the
+// reference's pileup cursor makes of them; needs_ref_has: K2's "reference has reads" bits need a buffer (depth's comes with its counters);
+// owes: several ranks with NCCL, the collective owed at the end of the run (a sparse run owes the sparse decision first).
+struct ModeNeeds { bool sub_batched, may_stage_sparse, loads_fprog, rewrites_lead_n, needs_ref_has; Owed owes; };
+constexpr ModeNeeds MODE_NEEDS[] = {      // indexed by RunMode
+    {true, true, true, true, false, Owed::BOUNDARY_TABLE}, /* RUN_FULL */           {false, false, true, true, false, Owed::NOTHING}, /* RUN_INFLATE_ONLY */
+    {false, false, true, false, true, Owed::NOTHING}, /* RUN_SCAN_ONLY */           {true, false, true, false, true, Owed::NOTHING}, /* RUN_INDEX */
+    {true, false, false, false, true, Owed::FLAGSTAT_SUM}, /* RUN_FLAGSTAT */       {true, true, false, false, true, Owed::VIEW_SUM}, /* RUN_VIEW_COUNT */
+    {true, true, false, false, true, Owed::VIEW_SUM}, /* RUN_VIEW_TEXT */
+};
+constexpr const char* MSG_PEER_STOPPED = "another rank of the run stopped with an error (its own message says why): no result";
+constexpr const char* MSG_CHUNK_MISMATCH = "the index does not describe this file (a region chunk does not end at a record)";
 constexpr int RC_RETRY_WINDOW = 1;      // internal: a read lies outside the counter window a multi-input run was given
+constexpr int RC_RESTART = 2;           // internal: the index does not describe the file; run_pipeline starts the run over without what it planned from it
 
 // ---- NCCL, bound at run time (dlopen) so that single-GPU users need no NCCL at all and so that a host
 // process that already loaded NCCL (e.g. through torch) shares that one instance (same SONAME).
@@ -158,11 +192,11 @@ struct bdepth {
     bool k3_pre = false;                  // BDEPTH_K3_PREFETCH=0: k3_gather without the lane-parallel record prefetch
     bool k3_tile = true;                  // BDEPTH_K3=gather: the round-1 per-position gather kernel instead of k3_tile
     bool has_fprog = false; FilterProg fprog; DevBuf fprog_d;      // -F: compiled query (filter.cuh); otherwise mapq_gt / flag_reject
-    DevBuf m_hash, m_flag, m_flt, m_ctl;
+    DevBuf m_hash, m_flag, m_ctl;
     uint32_t S = 1;                       // counter sets in the current run (samples, or 1)
     DevBuf rg_ids, rg_offs, rg_samp;
     DevBuf text[2], text_tiles, text_offs, text_zero, text_samp, present;
-    int coll_pending = 0;                 // several ranks: collectives of the current run this rank has not joined yet (2: the sparse decision and the boundary table; 1: the boundary table; 3: the all-reduce of the flagstat counters; 4: that of the view count) -- a rank that stops with an error joins them with a "failed" mark, so that the others stop too instead of waiting for it
+    Owed coll_pending = Owed::NOTHING;    // several ranks: the collective of the current run this rank owes its peers next (abort_collectives)
     bool want_presence = false;           // -a with -q and a positive minimum coverage: mark the positions reads cover (k_presence)
     uint64_t batch_u = 6ull << 30;
     uint64_t chunk_blocks = 13 * 32 * 16;              // BGZF blocks per H2D chunk = per K1 sub-launch = per sub-batch: 6656 blocks = 16 K1 CTAs, ~260 MB compressed
@@ -234,6 +268,9 @@ int fail(bdepth* h, int code, const char* fmt, ...) {
 }
 #define NK(call) do { int r__ = (call); if (r__ != 0) return fail(h, BDEPTH_ERR_NCCL, "NCCL error at %s:%d: %s", __FILE__, __LINE__, nccl().GetErrorString ? nccl().GetErrorString(r__) : "?"); } while (0)
 #define CK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return fail(h, BDEPTH_ERR_CUDA, "CUDA error %s at %s:%d: %s", cudaGetErrorName(e__), __FILE__, __LINE__, cudaGetErrorString(e__)); } while (0)
+// h->hs.up / down on the main stream, returning from the caller when the scratch is exhausted
+#define UP(dst, src, bytes) do { if (!h->hs.up(h->s_main, &h->st.gpu_launches, (dst), (src), (bytes))) return fail(h, BDEPTH_ERR_CUDA, "internal: host scratch exhausted"); } while (0)
+#define DOWN(var, type, src, bytes) type* var = (type*)h->hs.down(h->s_main, &h->st.gpu_launches, (src), (bytes)); if (!var) return fail(h, BDEPTH_ERR_CUDA, "internal: host scratch exhausted")
 
 int ensure_pinned(bdepth* h, size_t n) {
     if (n <= h->pinned_cap) return 0;
@@ -464,36 +501,53 @@ __global__ void k_add_u32(uint32_t* __restrict__ dst, const uint32_t* __restrict
 constexpr uint64_t PEER_FAILED = 0xFFFFFFFFFFFFFFFDull;      // in the boundary table instead of a rank's smallest start: that rank stopped with an error
 constexpr uint32_t SPARSE_PEER_FAILED = 1u << 16;            // the same in the sum of the sparse decision
 
-// A rank that stops with an error before the boundary table has been gathered still joins that all-gather (or, on a -L run, the decision
-// before it) and says so there: the other ranks then stop with an error of their own instead of waiting in the collective for ever (a
-// refusal such as "reads of one name reach too far past a shard boundary" concerns one rank only).  Best effort: errors in here are ignored.
+// flagstat's counters or view's count, each followed by one word that marks a failed rank in the all-reduce, and their host copy
+struct Census { DevBuf& d; uint64_t* host; size_t words; };
+Census census_of(bdepth* h, Owed sum) { return sum == Owed::FLAGSTAT_SUM ? Census{h->fs, h->fs_host, FS_WORDS + 1} : Census{h->vc, h->vc_host, 2}; }
+// flagstat / view at the end of a run: several ranks sum the counters and the "failed" words in one all-reduce (a rank that failed has joined
+// it through abort_collectives); the sum comes down to the host copy
+int finish_census(bdepth* h, Owed sum) {
+    const Census c = census_of(h, sum); cudaStream_t sm = h->s_main;
+    if (h->world > 1 && h->comm) { NK(nccl().AllReduce(c.d.p, c.d.p, c.words, NCCL_UINT64, NCCL_SUM, h->comm, sm)); h->coll_pending = Owed::NOTHING; }
+    CK(h->hs.ensure(16384)); h->hs.used = 0;      // (nothing is in flight: every sub-batch ended synchronised; a run without records has not sized it yet)
+    DOWN(p, uint64_t, c.d.p, c.words * 8); CK(cudaStreamSynchronize(sm)); memcpy(c.host, p, c.words * 8);
+    if (c.host[c.words - 1]) return fail(h, BDEPTH_ERR_NCCL, "%s", MSG_PEER_STOPPED);
+    return 0;
+}
+
+// A rank that stops with an error before the collectives of its run joins the one it owes (Owed) and says so there: the other ranks then stop
+// with an error of their own instead of waiting in the collective for ever (a refusal such as "reads of one name reach too far past a shard
+// boundary" concerns one rank only).  Best effort: errors in here are ignored.
 void abort_collectives(bdepth* h) {
-    const int p = h->coll_pending; h->coll_pending = 0;
-    if (!p || h->world <= 1 || !h->comm) return;
+    const Owed p = h->coll_pending; h->coll_pending = Owed::NOTHING;
+    if (p == Owed::NOTHING || h->world <= 1 || !h->comm) return;
     NcclApi& N = nccl(); cudaStream_t sm = h->s_main;
-    if (p == 3 || p == 4) {      // flagstat / view -c: the counters' all-reduce, with this rank's "failed" word set
-        uint64_t mark[FS_WORDS + 1] = {}; const size_t nw = p == 3 ? FS_WORDS + 1 : 2; mark[nw - 1] = 1;
-        DevBuf& d = p == 3 ? h->fs : h->vc;
-        if (d.ensure(nw * 8) != cudaSuccess) return;
-        cudaMemcpyAsync(d.p, mark, nw * 8, cudaMemcpyHostToDevice, sm);
-        N.AllReduce(d.p, d.p, nw, NCCL_UINT64, NCCL_SUM, h->comm, sm);
-        cudaStreamSynchronize(sm);
-        return;
+    switch (p) {
+        case Owed::FLAGSTAT_SUM: case Owed::VIEW_SUM: {      // the counters' all-reduce, with this rank's "failed" word set
+            const Census c = census_of(h, p); uint64_t mark[FS_WORDS + 1] = {}; mark[c.words - 1] = 1;
+            if (c.d.ensure(c.words * 8) != cudaSuccess) return;
+            cudaMemcpyAsync(c.d.p, mark, c.words * 8, cudaMemcpyHostToDevice, sm);
+            N.AllReduce(c.d.p, c.d.p, c.words, NCCL_UINT64, NCCL_SUM, h->comm, sm);
+            break;
+        }
+        case Owed::SPARSE_DECISION: {      // only that all-reduce: the others stop when they see the mark in its sum
+            uint32_t flag = SPARSE_PEER_FAILED;
+            if (h->misc.ensure(16) != cudaSuccess) return;
+            cudaMemcpyAsync(h->misc.p, &flag, 4, cudaMemcpyHostToDevice, sm);
+            N.AllReduce(h->misc.p, h->misc.p, 1, NCCL_UINT32, NCCL_SUM, h->comm, sm);
+            break;
+        }
+        case Owed::BOUNDARY_TABLE: {
+            DevBuf dpair, dall; if (dpair.ensure(16) != cudaSuccess || dall.ensure(16 * (size_t)h->world) != cudaSuccess) return;
+            uint64_t mine[2] = {PEER_FAILED, 0};
+            cudaMemcpyAsync(dpair.p, mine, 16, cudaMemcpyHostToDevice, sm);
+            N.AllGather(dpair.p, dall.p, 2, NCCL_UINT64, h->comm, sm);
+            cudaStreamSynchronize(sm); dpair.release(); dall.release();
+            return;
+        }
+        case Owed::NOTHING: return;
     }
-    if (p == 2) {
-        uint32_t flag = SPARSE_PEER_FAILED;
-        if (h->misc.ensure(16) != cudaSuccess) return;
-        cudaMemcpyAsync(h->misc.p, &flag, 4, cudaMemcpyHostToDevice, sm);
-        N.AllReduce(h->misc.p, h->misc.p, 1, NCCL_UINT32, NCCL_SUM, h->comm, sm);
-        cudaStreamSynchronize(sm);
-        return;
-    }
-    DevBuf dpair, dall; if (dpair.ensure(16) != cudaSuccess || dall.ensure(16 * (size_t)h->world) != cudaSuccess) return;
-    uint64_t mine[2] = {PEER_FAILED, 0};
-    cudaMemcpyAsync(dpair.p, mine, 16, cudaMemcpyHostToDevice, sm);
-    N.AllGather(dpair.p, dall.p, 2, NCCL_UINT64, h->comm, sm);
     cudaStreamSynchronize(sm);
-    dpair.release(); dall.release();
 }
 
 int exchange_boundaries(bdepth* h, uint64_t shard_min, uint64_t shard_max, bool with_counters) {
@@ -504,7 +558,7 @@ int exchange_boundaries(bdepth* h, uint64_t shard_min, uint64_t shard_max, bool 
     uint64_t mine[2] = {shard_min, shard_max};
     CK(cudaMemcpyAsync(dpair.p, mine, 16, cudaMemcpyHostToDevice, sm));
     NK(N.AllGather(dpair.p, dall.p, 2, NCCL_UINT64, h->comm, sm));
-    h->coll_pending = 0;
+    h->coll_pending = Owed::NOTHING;
     std::vector<uint64_t> all(2 * (size_t)W);
     CK(cudaMemcpyAsync(all.data(), dall.p, 16 * (size_t)W, cudaMemcpyDeviceToHost, sm));
     CK(cudaStreamSynchronize(sm));
@@ -730,200 +784,545 @@ int view_text_sub(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R
     return 0;
 }
 
-// The pipeline: leaves the per-position counters of the whole shard in h->counts (RUN_FULL).
-int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em);
-int run_pipeline(bdepth* h, RunMode mode, RunOut* ro, Emitter* em = nullptr) {
-    const int rc = run_pipeline_body(h, mode, ro, em);
-    if (rc && rc != RC_RETRY_WINDOW) abort_collectives(h);      // (a nested run -- the restarts below -- has done that itself: nothing is pending then)
-    return rc;
+// ---- the record pipeline: one front end shared by every run mode (H2D, K1 inflate, the K2 record-chain walk with its host verification,
+// K2 decode) hands each sub-batch of decoded records to the consumer of the run mode (the switch in run_pipeline_body).
+struct SubBatch {      // a sub-batch: R records decoded into soa from the inflated bytes at u0 (absolute offset batch_u0, ub bytes); ss: K2's statistics;
+    RecordSoA soa{}; uint8_t* u0 = nullptr; uint64_t R = 0, batch_u0 = 0, ub = 0; ScanStats ss{}; bool last_batch = false, last_sub = false; size_t batch_no = 0;
+    ScanParams sp{}; int64_t tail = 0, ghost_below = INT64_MIN; bool limited = false, mismatch = false;      // walk_records: tail = the first byte not consumed by a complete record, limited =
+};                                                                                  // records at or after the shard limit were dropped, mismatch = a region chunk's chain did not end at its end
+struct Pipe {                       // the state of one pipeline run that its steps share
+    bdepth* h; RunMode mode; RunOut* ro; Emitter* em;
+    bool sparse = false, fix = false;      // the blocks are the region query's BAI chunks (plan_sparse); -m
+    const std::vector<HostBlock>* B = nullptr; size_t blk_lo = 0, blk_hi = 0;
+    const FilterProg* d_fprog = nullptr; RgTable rgt{nullptr, nullptr, nullptr, 0};
+    uint32_t n_flt = 0;             // depth with -L: the merged regions in flt_d (starts, then ends), for k_ref_seen, the lead-N rewrite and the mates
+    std::vector<uint64_t> dco[2];   // dco[slot][i] = where block bb+i of the batch sits in comp2[slot] (see issue_h2d)
+    uint64_t carry_len = 0; bool first_batch = true; uint64_t shard_min = UINT64_MAX, shard_max = 0;
+    size_t ghost_b = 0; int64_t ghost_entry = 0; uint64_t ghost_below_abs = 0, prev_s_last = 0, covered_from = 0;      // -m: where the next batch's stream begins, what the mates carry on
+    bool census_timed = false; float ms_census = 0;      // flagstat / view -c: ev[22]..ev[23] of the sub-batch hold its census kernel
+};
+// H2D of blocks [bb, be) into comp2[slot]; waits until K1 of the batch that used the slot two batches ago is done.  Plain runs keep the file
+// layout (one copy per chunk); sparse runs pack the selected blocks back to back (one copy per run of file-adjacent blocks).
+int issue_h2d(Pipe& P, size_t no, size_t bb, size_t be) {
+    bdepth* h = P.h; const auto& B = *P.B; const bool sparse = P.sparse;
+    const int slot = (int)(no & 1);
+    uint64_t g0 = B[bb].coff & ~3ull;
+    if (no >= 2) CK(cudaStreamWaitEvent(h->s_copy, h->ev[16 + slot], 0));
+    CK(cudaEventRecord(h->ev[18 + slot], h->s_copy));
+    h->chunk_end[slot].clear();
+    auto& dco = P.dco[slot];
+    dco.resize(be - bb);
+    { uint64_t acc = 0; for (size_t i = bb; i < be; i++) { dco[i - bb] = sparse ? acc : B[i].coff - g0; acc += B[i].bsize; } }
+    size_t nch = 0;
+    for (size_t c0 = bb; c0 < be; c0 += h->chunk_blocks, nch++) {
+        size_t c1 = std::min<size_t>(be, c0 + h->chunk_blocks);
+        uint64_t dev_end;
+        if (!sparse) {
+            uint64_t a = c0 == bb ? g0 : B[c0].coff, e = B[c1 - 1].coff + B[c1 - 1].bsize;
+            CK(cudaMemcpyAsync((uint8_t*)h->comp2[slot].p + (a - g0), h->file + a, e - a, cudaMemcpyHostToDevice, h->s_copy));
+            dev_end = e - g0;
+        } else {
+            for (size_t r0 = c0; r0 < c1;) {
+                size_t r1 = r0 + 1; while (r1 < c1 && B[r1].coff == B[r1 - 1].coff + B[r1 - 1].bsize) r1++;
+                CK(cudaMemcpyAsync((uint8_t*)h->comp2[slot].p + dco[r0 - bb], h->file + B[r0].coff, B[r1 - 1].coff + B[r1 - 1].bsize - B[r0].coff, cudaMemcpyHostToDevice, h->s_copy));
+                r0 = r1;
+            }
+            dev_end = dco[c1 - 1 - bb] + B[c1 - 1].bsize;
+        }
+        if (c1 == be) CK(cudaMemsetAsync((uint8_t*)h->comp2[slot].p + dev_end, 0, 128, h->s_copy));
+        if (h->chunk_ev[slot].size() <= nch) { cudaEvent_t ne; CK(cudaEventCreateWithFlags(&ne, cudaEventDisableTiming)); h->chunk_ev[slot].push_back(ne); }
+        CK(cudaEventRecord(h->chunk_ev[slot][nch], h->s_copy));
+        h->chunk_end[slot].push_back(c1);
+    }
+    CK(cudaEventRecord(h->ev[14 + slot], h->s_copy));
+    return 0;
 }
+// K1 of blocks [c0, c0 + n) of the batch whose stream begins at block b, on stream ks: the two-phase inflater (k1_huff, k1_lz) and the exact
+// one-phase kernel for whatever phase 1 handed back (normally nothing: it returns at once); BDEPTH_K1_ONEPHASE=1 runs the round-1 kernel alone (A/B)
+int launch_k1(bdepth* h, cudaStream_t ks, const uint32_t* d_comp, uint8_t* u0, size_t b, size_t c0, uint32_t n) {
+    const BlockDesc* dd = h->descs.as<BlockDesc>() + (c0 - b); int* stp = h->status.as<int>() + (c0 - b);
+    if (h->k1_onephase) {
+        BD_LAUNCH((n + 32 * K1_WARPS - 1) / (32 * K1_WARPS), 32 * K1_WARPS, K1_SMEM, ks, k1_inflate)(d_comp, dd, n, u0, stp);
+        CK(cudaGetLastError()); h->st.gpu_launches++;
+        return 0;
+    }
+    BlockAux* ax = h->aux.as<BlockAux>() + (c0 - b); uint32_t* sgi = h->segi.as<uint32_t>() + (c0 - b) * MAX_SEG; uint8_t* ltb = h->littab.as<uint8_t>() + (c0 - b) * (size_t)MAX_SEG * 256;
+    const unsigned hg = (n + 32 * K1H_WARPS - 1) / (32 * K1H_WARPS); const uint32_t blk0 = (uint32_t)(c0 - b);
+#define K1H(LIMS, MINB) BD_LAUNCH(hg, 32 * K1H_WARPS, k1h_smem<LIMS>(), ks, k1_huff<LIMS, MINB>)(d_comp, dd, n, blk0, stp, h->tok.as<uint32_t>(), h->lits.as<uint8_t>(), ax, sgi, ltb)
+    // which instantiation: limits in registers at 4 CTAs per SM (16 warps) is the faster loop; when a launch has more warps than that
+    // holds at once (16 warps on every SM of the device), limits in shared memory at 5 CTAs (20 warps) wins by its occupancy
+    const int variant = h->k1h_variant >= 0 ? h->k1h_variant : (n > (uint32_t)h->n_sm * 16u * 32u ? 2 : 0);
+    switch (variant) { case 1: K1H(false, 6); break; case 2: K1H(true, 5); break; case 3: K1H(true, 4); break; default: K1H(false, 4); }
+#undef K1H
+    if (h->k1lz_flat) BD_LAUNCH((n + K1L_WARPS - 1) / K1L_WARPS, 32 * K1L_WARPS, 0, ks, k1_lz_flat)(dd, n, blk0, u0, stp, h->tok.as<uint32_t>(), h->lits.as<uint8_t>(), ax, sgi, ltb);
+    else if (h->k1lz_v12) BD_LAUNCH((n + K1L_WARPS - 1) / K1L_WARPS, 32 * K1L_WARPS, 0, ks, k1_lz<false>)(dd, n, blk0, u0, stp, h->tok.as<uint32_t>(), h->lits.as<uint8_t>(), ax, sgi, ltb);
+    else BD_LAUNCH((n + K1L_WARPS - 1) / K1L_WARPS, 32 * K1L_WARPS, 0, ks, k1_lz<true>)(dd, n, blk0, u0, stp, h->tok.as<uint32_t>(), h->lits.as<uint8_t>(), ax, sgi, ltb);
+    BD_LAUNCH((n + 32 * K1_WARPS - 1) / (32 * K1_WARPS), 32 * K1_WARPS, K1_SMEM, ks, k1_fallback)(d_comp, dd, n, u0, stp);
+    CK(cudaGetLastError()); h->st.gpu_launches += 3;
+    return 0;
+}
+// ---- depth: the counter window (28 B/position) and the per-reference "has reads" bits.  With a BAI the linear index bounds where reads can lie, so only
+// that span of the linear genome is allocated; without one the whole genome is (87 GB for GRCh38: more than an 80 GB H100 holds, so BDEPTH_ERR_CUDA below).
+int setup_counter_window(Pipe& P) {
+    bdepth* h = P.h; const auto& B = *P.B; const size_t nref = h->hdr.ref_len.size(); cudaStream_t sm = h->s_main;
+    if (h->accum) return 0;      // a further input of the same run: counters, window, sample planes stay as the first input left them
+    uint64_t lo = 0, hi = h->hdr.total_len;
+    if (h->force_window) { lo = h->cnt_base; hi = h->cnt_base + h->win_len; }
+    else
+    if (h->bai.valid && h->bai_window_ok && h->bai.ioffsets.size() == nref && h->world > 1 && !P.sparse && !P.fix && P.blk_hi > P.blk_lo) {
+        // a shard: from the window in which its first record begins (its own positions begin there or later) to the end of the last
+        // 16 kbp window that any read before the shard's end overlaps (the linear index holds, per window, the first such read)
+        const uint64_t vo_end = P.blk_hi < B.size() ? (B[P.blk_hi].coff << 16) : (h->file_len << 16);
+        lo = h->rank == 0 ? UINT64_MAX : h->zone_lin_lo; hi = 0;
+        for (size_t r = 0; r < nref; r++) {
+            const auto& v = h->bai.ioffsets[r];
+            for (size_t k = 0; k < v.size(); k++) if (v[k] && v[k] < vo_end) {
+                const uint64_t a = h->hdr.ref_lin0[r] + std::min<uint64_t>((uint64_t)k << 14, h->hdr.ref_len[r]), e = h->hdr.ref_lin0[r] + std::min<uint64_t>((uint64_t)(k + 1) << 14, h->hdr.ref_len[r]);
+                if (h->rank == 0) lo = std::min(lo, a);
+                if (e > hi) hi = e;
+            }
+        }
+        if (lo == UINT64_MAX || lo >= hi) { lo = 0; hi = h->hdr.total_len; }
+    } else if (h->bai.valid && h->bai_window_ok && h->bai.ioffsets.size() == nref && h->world == 1) {
+        lo = UINT64_MAX; hi = 0;
+        for (size_t r = 0; r < nref; r++) {
+            const auto& v = h->bai.ioffsets[r]; if (v.empty()) continue;
+            size_t k = 0; while (k < v.size() && v[k] == 0) k++;
+            if (k == v.size()) continue;
+            lo = std::min<uint64_t>(lo, h->hdr.ref_lin0[r] + std::min<uint64_t>((uint64_t)k << 14, h->hdr.ref_len[r]));
+            hi = std::max<uint64_t>(hi, h->hdr.ref_lin0[r] + std::min<uint64_t>((uint64_t)v.size() << 14, h->hdr.ref_len[r]));
+        }
+        if (lo >= hi) { lo = 0; hi = h->hdr.total_len; }      // an index without linear entries says nothing
+    }
+    if (!h->force_window) {
+        h->cnt_base = lo / TILE_POS * TILE_POS;
+        h->win_len = ((hi - h->cnt_base + TILE_POS - 1) / TILE_POS + 1) * TILE_POS;
+    }
+    h->S = (h->combined || h->hdr.sample_names.size() <= 1) ? 1u : (uint32_t)h->hdr.sample_names.size();
+    if (h->S > 64) return fail(h, BDEPTH_ERR_ARG, "%u samples: per-sample output supports at most 64 (use --combined)", h->S);
+    size_t need = (size_t)h->win_len * N_PLANES * 4 * h->S;
+    size_t free_b = 0, tot_b = 0; CK(cudaMemGetInfo(&free_b, &tot_b));
+    if (need > h->counts.cap && need > free_b + h->counts.cap) return fail(h, BDEPTH_ERR_CUDA, "counter window needs %zu bytes of HBM, %zu free", need, free_b);
+    CK(h->counts.ensure(need));
+    CK(cudaMemsetAsync(h->counts.p, 0, need, sm));
+    if (h->want_presence) { CK(h->present.ensure((h->win_len / 32 + 2) * 4)); CK(cudaMemsetAsync(h->present.p, 0, (h->win_len / 32 + 2) * 4, sm)); }
+    CK(h->ref_has.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has.p, 0, (nref / 32 + 2) * 4, sm));
+    return 0;
+}
+// depth: the @RG ID -> sample table for the per-read RG lookup (depth.d:240-250); mates pair within a sample
+int upload_rg_table(Pipe& P) {
+    bdepth* h = P.h; cudaStream_t sm = h->s_main;
+    if (!(h->S > 1 || (P.fix && h->hdr.sample_names.size() > 1))) return 0;
+    std::vector<uint8_t> ids; std::vector<uint32_t> offs; std::vector<uint8_t> samp;
+    for (size_t g = 0; g < h->hdr.rg_ids.size(); g++) { offs.push_back((uint32_t)ids.size()); ids.insert(ids.end(), h->hdr.rg_ids[g].begin(), h->hdr.rg_ids[g].end()); ids.push_back(0); samp.push_back((uint8_t)h->hdr.rg_sample[g]); }
+    CK(h->rg_ids.ensure(ids.size() + 8)); CK(h->rg_offs.ensure(offs.size() * 4 + 8)); CK(h->rg_samp.ensure(samp.size() + 8));
+    CK(cudaMemcpyAsync(h->rg_ids.p, ids.data(), ids.size(), cudaMemcpyHostToDevice, sm)); CK(cudaMemcpyAsync(h->rg_offs.p, offs.data(), offs.size() * 4, cudaMemcpyHostToDevice, sm)); CK(cudaMemcpyAsync(h->rg_samp.p, samp.data(), samp.size(), cudaMemcpyHostToDevice, sm));
+    CK(cudaStreamSynchronize(sm));
+    P.rgt = RgTable{h->rg_ids.as<uint8_t>(), h->rg_offs.as<uint32_t>(), h->rg_samp.as<uint8_t>(), (uint32_t)offs.size()};
+    return 0;
+}
+// depth with -L: the merged regions (sorted, disjoint) in linear coordinates, starts then ends, once per run; K2's every-passing-read bits
+// go to a scratch word array, k_ref_seen marks the references of the reads that overlap a region
+int upload_regions(Pipe& P) {
+    bdepth* h = P.h; cudaStream_t sm = h->s_main; const size_t nref = h->hdr.ref_len.size();
+    P.n_flt = (uint32_t)h->regions.size();
+    if (!P.n_flt) return 0;
+    std::vector<uint64_t> fl; fl.reserve(2 * (size_t)P.n_flt);
+    for (auto& g : h->regions) fl.push_back(h->hdr.ref_lin0[g.ref_id] + g.start);
+    for (auto& g : h->regions) fl.push_back(h->hdr.ref_lin0[g.ref_id] + g.end);
+    CK(h->flt_d.ensure(fl.size() * 8)); CK(cudaMemcpyAsync(h->flt_d.p, fl.data(), fl.size() * 8, cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm));      // (fl is a local)
+    CK(h->ref_has_all.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has_all.p, 0, (nref / 32 + 2) * 4, sm));
+    return 0;
+}
+// index: the tables of k_index_scan -- one linear-index row per reference (16 kbp windows up to one past the reference end), counters, carry
+int setup_index_tables(bdepth* h) {
+    const size_t nref = h->hdr.ref_len.size(); cudaStream_t sm = h->s_main;
+    auto& X = h->ix; X.base.assign(nref + 1, 0); X.cap.assign(nref + 1, 0); uint64_t acc = 0;
+    for (size_t r = 0; r < nref; r++) { X.base[r] = (uint32_t)acc; X.cap[r] = (uint32_t)std::min<uint64_t>(32769, ((uint64_t)h->hdr.ref_len[r] >> 14) + 2); acc += X.cap[r]; if (acc > 0xFFFFFFF0ull) return fail(h, BDEPTH_ERR_ARG, "too many references for the linear index tables"); }
+    X.n_lin = acc; X.h_runs.clear(); X.h_excs.clear();
+    CK(X.lin.ensure((acc + 1) * 8)); CK(X.lin_len.ensure((nref + 1) * 4)); CK(X.lin_base.ensure((nref + 1) * 4)); CK(X.lin_cap.ensure((nref + 1) * 4));
+    CK(X.n_mapped.ensure((nref + 1) * 8)); CK(X.n_unmapped.ensure((nref + 1) * 8)); CK(X.carry.ensure(sizeof(IndexCarry))); CK(X.ctl.ensure(sizeof(IndexCtl)));
+    CK(cudaMemsetAsync(X.lin.p, 0xFF, (acc + 1) * 8, sm)); CK(cudaMemsetAsync(X.lin_len.p, 0, (nref + 1) * 4, sm)); CK(cudaMemsetAsync(X.n_mapped.p, 0, (nref + 1) * 8, sm)); CK(cudaMemsetAsync(X.n_unmapped.p, 0, (nref + 1) * 8, sm));
+    CK(cudaMemsetAsync(X.carry.p, 0, sizeof(IndexCarry), sm));
+    CK(cudaMemcpyAsync(X.lin_base.p, X.base.data(), (nref + 1) * 4, cudaMemcpyHostToDevice, sm)); CK(cudaMemcpyAsync(X.lin_cap.p, X.cap.data(), (nref + 1) * 4, cudaMemcpyHostToDevice, sm));
+    IndexCtl c0{0, 0, 0, ~0ull, ~0ull, 0, ~0ull, 0};
+    CK(cudaMemcpyAsync(X.ctl.p, &c0, sizeof c0, cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm));
+    return 0;
+}
+// ---- K2 of the sub-batch [b, b1) (inflate status `stt`): chunk table, walk, exact chain verification on the host, and the shard-limit trim
+int walk_records(Pipe& P, SubBatch& s, size_t b, size_t b1, const int* stt) {
+    bdepth* h = P.h; const auto& B = *P.B; const bool sparse = P.sparse, fix = P.fix; cudaStream_t sm = h->s_main; bdepth_stats& st = h->st;
+    const size_t nb = b1 - b; const uint64_t batch_u0 = s.batch_u0, ub = s.ub;
+    const bool seg0 = sparse && h->seg_entry[b] >= 0;      // the sub-batch begins a new region-query chunk: nothing is carried into it
+    if (seg0) P.carry_len = 0;
+    const uint64_t carry_len = P.carry_len;
+    std::vector<int64_t> cstart(nb + 1); std::vector<uint32_t> sbase(nb + 1);
+    { uint64_t acc = 0; for (size_t i = 0; i < nb; i++) { cstart[i] = (int64_t)(B[b + i].uoff - batch_u0); sbase[i] = (uint32_t)acc; uint64_t sz = B[b + i].isize + (i == 0 ? carry_len : 0); acc += sz / 36 + 2; } cstart[nb] = (int64_t)ub; sbase[nb] = (uint32_t)acc; cstart[0] = -(int64_t)carry_len;
+      if (acc > 0xFFFFFFFFull) return fail(h, BDEPTH_ERR_ARG, "batch too large"); }
+    const uint64_t n_slots = sbase[nb];
+    CK(h->chunk_start.ensure((nb + 1) * 8)); CK(h->slot_base.ensure((nb + 1) * 4)); CK(h->entry.ensure(nb * 8)); CK(h->exitb.ensure(nb * 8)); CK(h->count.ensure(nb * 4)); CK(h->rec_base.ensure((nb + 1) * 4)); CK(h->slots.ensure(n_slots * 2 + 64)); CK(h->walk_list.ensure(64));
+    UP(h->chunk_start.p, cstart.data(), (nb + 1) * 8);
+    UP(h->slot_base.p, sbase.data(), (nb + 1) * 4);
+    CK(cudaMemsetAsync(h->entry.p, ENTRY_NONE_BYTE, nb * 8, sm));
+    // (-m: a stream that begins exactly where a region-query chunk begins starts at that chunk's first record)
+    int64_t anchor = (fix && s.batch_no > 0) ? ((seg0 && P.ghost_entry < (int64_t)h->seg_entry[b]) ? (int64_t)h->seg_entry[b] : P.ghost_entry) : seg0 ? (int64_t)h->seg_entry[b] : P.first_batch ? h->entry0 : -(int64_t)carry_len;
+    UP(h->entry.p, &anchor, 8);
+    CK(cudaMemsetAsync(h->misc.p, 0, 64, sm));
+    // records that START at or after the shard limit belong to the next rank
+    int64_t u_limit = (int64_t)ub; if (!sparse && h->limit_abs_u < batch_u0 + ub) u_limit = (int64_t)h->limit_abs_u - (int64_t)batch_u0;      // may be negative: the limit lies before this sub-batch, and a carried record that starts at or after it is not ours either
+    s.sp = ScanParams{s.u0, -(int64_t)carry_len, (int64_t)ub, (int)h->hdr.ref_len.size(), h->ref_len_d.as<uint32_t>(), h->ref_lin0_d.as<uint64_t>()};
+    const ScanParams& sp = s.sp;
+    BD_LAUNCH((unsigned)((nb * 32 + 255) / 256), 256, 0, sm, k2_guess_entries)(sp, h->chunk_start.as<int64_t>(), (uint32_t)nb, h->entry.as<int64_t>());
+    CK(cudaGetLastError()); st.gpu_launches++;
+    const int64_t* d_limit = nullptr;
+    if (sparse) {       // chunks of the region query: exact entries at their first blocks, walk limits at their last ones
+        std::vector<uint32_t> ai; std::vector<int64_t> av; std::vector<int64_t> lim(nb, INT64_MAX);
+        for (size_t i = 0; i < nb; i++) {
+            if (i && h->seg_entry[b + i] >= 0) { ai.push_back((uint32_t)i); av.push_back(cstart[i] + h->seg_entry[b + i]); }
+            if (h->seg_limit[b + i] != UINT32_MAX) lim[i] = (i ? cstart[i] : 0) + (int64_t)h->seg_limit[b + i];
+        }
+        CK(h->chunk_limit.ensure(nb * 8)); UP(h->chunk_limit.p, lim.data(), nb * 8); d_limit = h->chunk_limit.as<int64_t>();
+        if (!ai.empty()) {
+            CK(h->anchors_idx.ensure(ai.size() * 4)); CK(h->anchors_val.ensure(av.size() * 8));
+            UP(h->anchors_idx.p, ai.data(), ai.size() * 4); UP(h->anchors_val.p, av.data(), av.size() * 8);
+            BD_LAUNCH((unsigned)((ai.size() + 255) / 256), 256, 0, sm, k_scatter_i64)(h->entry.as<int64_t>(), h->anchors_idx.as<uint32_t>(), h->anchors_val.as<int64_t>(), (uint32_t)ai.size());
+            CK(cudaGetLastError()); st.gpu_launches++;
+        }
+    }
+    BD_LAUNCH((unsigned)((nb + 127) / 128), 128, 0, sm, k2_walk)(sp, h->chunk_start.as<int64_t>(), (uint32_t)nb, h->entry.as<int64_t>(), h->slot_base.as<uint32_t>(), h->slots.as<uint16_t>(), h->count.as<uint32_t>(), h->exitb.as<int64_t>(), (int*)h->misc.p, nullptr, 0, d_limit);
+    CK(cudaGetLastError()); st.gpu_launches++;
+    DOWN(ent, int64_t, h->entry.p, nb * 8); DOWN(ext, int64_t, h->exitb.p, nb * 8); DOWN(cnt, uint32_t, h->count.p, nb * 4);      // host-owned once synchronised
+    DOWN(werr, int, h->misc.p, 4);
+    CK(cudaStreamSynchronize(sm));
+    int walk_err = *werr;
+    for (size_t i = 0; i < nb; i++) if (stt[i]) return fail(h, BDEPTH_ERR_FORMAT, "DEFLATE error %d in BGZF block at offset %llu", stt[i], (unsigned long long)B[b + i].coff);
+    // ---- exact chain verification (host, control plane): entry[i] must equal the running exit
+    int64_t cur = anchor;
+    for (size_t i = 0; i < nb; i++) {
+        if (sparse && i && h->seg_entry[b + i] >= 0) cur = cstart[i] + h->seg_entry[b + i];     // a new chunk: the chain restarts at its first record
+        int64_t true_e = (cur < cstart[i + 1]) ? cur : ENTRY_NONE;
+        if (true_e != ENTRY_NONE && true_e < cstart[i]) return fail(h, BDEPTH_ERR_FORMAT, "internal: record chain went backwards");
+        if (ent[i] != true_e) {
+            st.chain_fixups++;
+            uint32_t ci = (uint32_t)i;
+            UP((int64_t*)h->entry.p + i, &true_e, 8);
+            UP(h->walk_list.p, &ci, 4);
+            BD_LAUNCH(1, 32, 0, sm, k2_walk)(sp, h->chunk_start.as<int64_t>(), (uint32_t)nb, h->entry.as<int64_t>(), h->slot_base.as<uint32_t>(), h->slots.as<uint16_t>(), h->count.as<uint32_t>(), h->exitb.as<int64_t>(), (int*)h->misc.p, h->walk_list.as<uint32_t>(), 1, d_limit);
+            CK(cudaGetLastError()); st.gpu_launches++;
+            DOWN(fx_ext, int64_t, (int64_t*)h->exitb.p + i, 8); DOWN(fx_cnt, uint32_t, (uint32_t*)h->count.p + i, 4); DOWN(fx_err, int, h->misc.p, 4);
+            CK(cudaStreamSynchronize(sm));
+            ext[i] = *fx_ext; cnt[i] = *fx_cnt; walk_err = *fx_err;
+            ent[i] = true_e;
+        }
+        if (true_e != ENTRY_NONE) {
+            cur = ext[i];
+            if (sparse && h->seg_limit[b + i] != UINT32_MAX) {      // last block of a chunk: the chain must end exactly at the chunk end
+                if (ext[i] != (i ? cstart[i] : 0) + (int64_t)h->seg_limit[b + i]) { s.mismatch = true; return 0; }
+                cur = INT64_MAX / 2;                                  // nothing follows until the next chunk begins
+                continue;
+            }
+            if (ext[i] < cstart[i + 1]) {      // the walk stopped inside its own block: incomplete tail record
+                for (size_t j = i + 1; j < nb; j++) cnt[j] = 0;
+                break;
+            }
+        }
+    }
+    if (walk_err) return fail(h, BDEPTH_ERR_FORMAT, "corrupt BAM record chain (block_size < 32)");
+    s.tail = cur < (int64_t)ub ? cur : (int64_t)ub;      // ---- shard limit: drop records starting at/after u_limit (host trims counts; offsets are sorted)
+    std::vector<uint32_t> rbase(nb + 1); uint64_t R = 0;
+    s.limited = u_limit < (int64_t)ub && !fix;        // (-m keeps the records behind the limit: they are marked as the next rank's by k2_decode)
+    std::vector<uint16_t> tmp_slots;
+    for (size_t i = 0; i < nb; i++) {
+        if (s.limited && cnt[i]) {
+            if (cstart[i] >= u_limit) cnt[i] = 0;
+            else if (cstart[i + 1] > u_limit) {   // partial: count slots below the limit
+                tmp_slots.resize(cnt[i]);
+                CK(cudaMemcpy(tmp_slots.data(), (uint16_t*)h->slots.p + sbase[i], cnt[i] * 2, cudaMemcpyDeviceToHost));
+                uint32_t k = 0; while (k < cnt[i] && ((k == 0 || cstart[i] > 0) ? cstart[i] : 0) + tmp_slots[k] < u_limit) k++;     // slot encoding: see k2_walk
+                cnt[i] = k;
+            }
+        }
+        rbase[i] = (uint32_t)R; R += cnt[i];
+    }
+    rbase[nb] = (uint32_t)R;
+    if (R > 0xFFFFFFF0ull) return fail(h, BDEPTH_ERR_ARG, "batch too large");
+    UP(h->count.p, cnt, nb * 4);
+    if (s.limited && s.last_batch && s.tail < u_limit && s.tail < (int64_t)ub && b1 < B.size()) return fail(h, BDEPTH_ERR_FORMAT, "record at the shard boundary spans more than %u BGZF blocks", SHARD_EXTRA_BLOCKS);
+    UP(h->rec_base.p, rbase.data(), (nb + 1) * 4);
+    st.n_records += R; s.R = R; return 0;
+}
+// ---- K2 decode of the walked records into s.soa, the lead-N rewrite and k_ref_seen; s.ss gets K2's statistics
+int decode_records(Pipe& P, SubBatch& s, size_t nb) {
+    bdepth* h = P.h; const bool fix = P.fix; cudaStream_t sm = h->s_main; bdepth_stats& st = h->st; const size_t nref = h->hdr.ref_len.size();
+    const uint64_t R = s.R, batch_u0 = s.batch_u0; const ModeNeeds& need = MODE_NEEDS[P.mode];
+    const size_t Rc = R ? R : 1;
+    CK(h->soa_start.ensure(Rc * 8)); CK(h->soa_span.ensure(Rc * 4)); CK(h->soa_meta.ensure(Rc * 4)); CK(h->soa_off.ensure(Rc * 8)); CK(h->soa_ncl.ensure(Rc * 4)); CK(h->soa_lseq.ensure(Rc * 4)); CK(h->long_list.ensure(Rc * 4));
+    const RecordSoA soa = s.soa = RecordSoA{h->soa_start.as<uint64_t>(), h->soa_span.as<uint32_t>(), h->soa_meta.as<uint32_t>(), h->soa_off.as<int64_t>(), h->soa_ncl.as<uint32_t>(), h->soa_lseq.as<int32_t>()};
+    ScanStats zs{0, 0, 0, 0, ~0ull, 0, 0, ~0ull, 0, 0, ~0ull, 0, ~0ull, ~0ull, 0};
+    const int64_t ghost_below = s.ghost_below = (fix && s.batch_no > 0) ? (int64_t)P.ghost_below_abs - (int64_t)batch_u0 : INT64_MIN;      // (-m: the consumer's mates use it too)
+    const int64_t own_lo = (fix && h->world > 1) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;           // -m on several ranks: records outside belong to the neighbours
+    const int64_t own_hi = (fix && h->world > 1 && h->limit_abs_u < h->total_u) ? (int64_t)h->limit_abs_u - (int64_t)batch_u0 : INT64_MAX;
+    const int64_t zone_below = (!fix && !P.sparse && h->world > 1) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;       // records of the previous ranks' zone
+    UP(h->scan_stats.p, &zs, sizeof zs);
+    if (need.needs_ref_has && !h->ref_has.p) { CK(h->ref_has.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has.p, 0, (nref / 32 + 2) * 4, sm)); }
+    uint32_t* has_dst = P.n_flt ? h->ref_has_all.as<uint32_t>() : h->ref_has.as<uint32_t>();      // (-L: k_ref_seen below sets ref_has)
+    const ScanParams& sp = s.sp; const FilterProg* d_fprog = P.d_fprog;
+#define K2_DECODE(F, G) BD_LAUNCH((unsigned)((nb * 32 + 255) / 256), 256, 0, sm, k2_decode<F, G>)(sp, h->chunk_start.as<int64_t>(), (uint32_t)nb, h->slot_base.as<uint32_t>(), h->slots.as<uint16_t>(), h->count.as<uint32_t>(), h->rec_base.as<uint32_t>(), soa, h->mapq_gt, h->flag_reject, h->scan_stats.as<ScanStats>(), h->long_list.as<uint32_t>(), has_dst, P.rgt, d_fprog, ghost_below, own_lo, own_hi, zone_below)
+    if (fix) { if (d_fprog) K2_DECODE(true, true); else K2_DECODE(false, true); }
+    else if (d_fprog) K2_DECODE(true, false);
+    else K2_DECODE(false, false);
+#undef K2_DECODE
+    CK(cudaGetLastError()); st.gpu_launches++;
+    if (R && need.rewrites_lead_n) {      // quirk 1: CIGARs that begin with N, rewritten to what the reference's cursor makes of them (the index, the raw scan, flagstat and view see the file as it is)
+        // region mode proper (no window slots, no -m, one rank): the statistics of such a read are reproduced (kernels.cuh); otherwise refused
+        const bool lead_n_regions = h->seg.on && h->seg.n && !h->seg.has_u && !h->seg.has_min && !fix && h->world == 1;
+        LeadNSegs lsg{nullptr, nullptr, nullptr, nullptr, 0u, nullptr, nullptr, 1u, h->minq};
+        if (lead_n_regions) lsg = LeadNSegs{h->seg.s.as<uint64_t>(), h->seg.e.as<uint64_t>(), h->seg.pmax.as<uint64_t>(), h->seg.id.as<uint32_t>(), h->seg.n, h->seg.reads.as<uint32_t>(), h->seg.mbases.as<uint32_t>(),
+                                            (uint32_t)((h->combined || h->hdr.sample_names.size() <= 1) ? 1 : h->hdr.sample_names.size()), h->minq};
+        CK(h->lead_list.ensure(Rc * 4));
+        BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k2_lead_n_find)(soa, s.u0, (uint32_t)R, h->lead_list.as<uint32_t>(), h->scan_stats.as<ScanStats>());
+        BD_LAUNCH(32, 128, 0, sm, k2_lead_n_fix)(soa, s.u0, h->lead_list.as<uint32_t>(), h->scan_stats.as<ScanStats>(), (h->seg.on && !lead_n_regions) ? 1 : 0,
+                                                P.n_flt ? h->flt_d.as<uint64_t>() : nullptr, P.n_flt ? h->flt_d.as<uint64_t>() + P.n_flt : nullptr, P.n_flt, lsg);
+        CK(cudaGetLastError()); st.gpu_launches += 2;
+    }
+    if (P.n_flt && R) {
+        BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_ref_seen)(soa, (uint32_t)R, h->flt_d.as<uint64_t>(), h->flt_d.as<uint64_t>() + P.n_flt, P.n_flt, h->ref_lin0_d.as<uint64_t>(), (uint32_t)nref, h->ref_has.as<uint32_t>());
+        CK(cudaGetLastError()); st.gpu_launches++;
+    }
+    DOWN(ssp, ScanStats, h->scan_stats.p, sizeof(ScanStats));
+    CK(cudaEventRecord(h->ev[3], sm)); CK(cudaStreamSynchronize(sm));
+    const ScanStats& ss = s.ss = *ssp;
+    st.n_records -= ss.n_ghost + ss.n_ghost_right;          // re-read records of the previous batch / of the neighbours' zones are counted there
+    if (ss.bad_rec != ~0ull) return fail(h, BDEPTH_ERR_FORMAT, "corrupt BAM record (#%llu of the batch): its name, CIGAR, sequence and qualities do not fit its block_size", ss.bad_rec);
+    if (ss.lead_n != ~0ull) return fail(h, BDEPTH_ERR_FORMAT, "read #%llu of the batch: its CIGAR begins with N%s (pileup.d:180-189): there is no result to reproduce", ss.lead_n,
+                                         h->seg.on ? " -- the reference computes region / window statistics of such a read partly from its CIGAR as written and partly from a cursor that skips the leading N" : " and ends in a match -- the reference's pileup cursor runs past the read's sequence on such a read");
+    if (ss.rg_err != ~0ull) return fail(h, BDEPTH_ERR_FORMAT, "error in read #%llu of the batch: its read group is not present in the header", ss.rg_err);
+    st.n_records_pass += ss.n_pass; st.n_cigar_ops += ss.n_cigar; st.seq_bytes += ss.seq_bytes; st.long_reads += ss.n_long;
+    if (ss.n_pass) { P.shard_min = std::min<uint64_t>(P.shard_min, ss.min_start); P.shard_max = std::max<uint64_t>(P.shard_max, ss.max_end); }
+    return 0;
+}
+// ---- consumers: what each run mode does with a sub-batch.  Each records ev[4], the end of its coverage time (ms_coverage): after its own work,
+// or before it where that work is timed on its own (ms_reduce).
+// scan_to_host: the records' fields, copied out
+int consume_scan(Pipe& P, const SubBatch& s) {
+    bdepth* h = P.h; RunOut* ro = P.ro; const size_t nref = h->hdr.ref_len.size(); const RecordSoA& soa = s.soa; const uint64_t R = s.R;
+    if (ro && R) {
+        uint64_t n = std::min<uint64_t>(R, ro->scan_cap > ro->scan_n ? ro->scan_cap - ro->scan_n : 0);
+        std::vector<uint64_t> hs(n), ho(n); std::vector<uint32_t> hsp(n), hm(n), hn(n);
+        CK(cudaMemcpy(hs.data(), soa.start, n * 8, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(ho.data(), soa.off, n * 8, cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(hsp.data(), soa.span, n * 4, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(hm.data(), soa.meta, n * 4, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(hn.data(), soa.ncl, n * 4, cudaMemcpyDeviceToHost));
+        for (uint64_t i = 0; i < n; i++) {
+            uint64_t k = ro->scan_n + i; int32_t rid = -1, p = -1;
+            if (hs[i] != START_UNPLACED) { size_t lo = 0, hi = nref; while (lo + 1 < hi) { size_t m = (lo + hi) / 2; if (h->hdr.ref_lin0[m] <= hs[i]) lo = m; else hi = m; } while (lo + 1 < nref && h->hdr.ref_lin0[lo + 1] <= hs[i] && h->hdr.ref_len[lo] == 0) lo++; rid = (int32_t)lo; p = (int32_t)(hs[i] - h->hdr.ref_lin0[lo]); }
+            if (ro->ref_id) ro->ref_id[k] = rid; if (ro->pos) ro->pos[k] = p; if (ro->span) ro->span[k] = hsp[i];
+            if (ro->flag) ro->flag[k] = (uint16_t)(hm[i] >> 16); if (ro->mapq) ro->mapq[k] = (uint8_t)(hm[i] >> 8); if (ro->n_cigar) ro->n_cigar[k] = (uint16_t)(hn[i] >> 8);
+            if (ro->rec_off) ro->rec_off[k] = s.batch_u0 + ho[i] - 4;       // absolute offset of the block_size field
+        }
+    }
+    if (ro) ro->scan_n += R;
+    CK(cudaEventRecord(h->ev[4], h->s_main)); return 0;
+}
+// BAI builder: the per-record part of IndexBuilder.put (bai/indexing.d:290-333) for the sub-batch's records
+int consume_index(Pipe& P, const SubBatch& s) {
+    bdepth* h = P.h; cudaStream_t sm = h->s_main; const uint64_t R = s.R;
+    if (R) {
+        auto& X = h->ix;
+        CK(X.runs.ensure(R * sizeof(IndexRun))); CK(X.excs.ensure(R * sizeof(IndexExc)));
+        BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_index_scan)(s.soa, s.u0, (uint32_t)R, (unsigned long long)s.batch_u0, (int)h->hdr.ref_len.size(), X.lin_base.as<uint32_t>(), X.lin_cap.as<uint32_t>(), X.lin.as<unsigned long long>(), X.lin_len.as<uint32_t>(),
+                                                                           X.n_mapped.as<unsigned long long>(), X.n_unmapped.as<unsigned long long>(), X.carry.as<IndexCarry>(), X.runs.as<IndexRun>(), X.excs.as<IndexExc>(), X.ctl.as<IndexCtl>());
+        BD_LAUNCH(1, 32, 0, sm, k_index_carry)(s.soa, s.u0, (unsigned long long)s.batch_u0, X.carry.as<IndexCarry>(), X.ctl.as<IndexCtl>());
+        CK(cudaGetLastError()); h->st.gpu_launches += 2;
+        DOWN(icp, IndexCtl, X.ctl.p, sizeof(IndexCtl));
+        CK(cudaStreamSynchronize(sm));
+        const IndexCtl ic = *icp;
+        if (ic.bad_ref != ~0ull) return fail(h, BDEPTH_ERR_FORMAT, "record #%llu of the batch names a reference the header does not have", ic.bad_ref);
+        if (ic.unsorted != ~0ull) return fail(h, BDEPTH_ERR_FORMAT, "BAM file is not coordinate-sorted (record #%llu of the batch lies before the read in front of it)", ic.unsorted);
+        if (ic.past_end) return fail(h, BDEPTH_ERR_FORMAT, "%llu reads reach more than 16 kbp past the end of their reference: no index is built for such a file", ic.past_end);
+        if (ic.n_runs) { size_t o = X.h_runs.size(); X.h_runs.resize(o + ic.n_runs); CK(cudaMemcpy(X.h_runs.data() + o, X.runs.p, ic.n_runs * sizeof(IndexRun), cudaMemcpyDeviceToHost)); std::sort(X.h_runs.begin() + o, X.h_runs.end(), [](const IndexRun& a, const IndexRun& b) { return a.start_abs < b.start_abs; }); }
+        if (ic.n_exc) { size_t o = X.h_excs.size(); X.h_excs.resize(o + ic.n_exc); CK(cudaMemcpy(X.h_excs.data() + o, X.excs.p, ic.n_exc * sizeof(IndexExc), cudaMemcpyDeviceToHost)); std::sort(X.h_excs.begin() + o, X.h_excs.end(), [](const IndexExc& a, const IndexExc& b) { return a.start_abs < b.start_abs; }); }
+        CK(cudaMemsetAsync(X.ctl.p, 0, 16, sm));      // n_runs, n_exc
+    }
+    CK(cudaEventRecord(h->ev[4], sm)); return 0;
+}
+// depth: per-read segment counting, K3, -m's mates, the progressive delivery of finished positions; a read outside the counter window restarts the run.
+int consume_depth(Pipe& P, const SubBatch& s, size_t n_subs) {
+    bdepth* h = P.h; const auto& B = *P.B; const bool fix = P.fix; cudaStream_t sm = h->s_main; bdepth_stats& st = h->st;
+    const RecordSoA& soa = s.soa; uint8_t* const u0 = s.u0; const uint64_t R = s.R, batch_u0 = s.batch_u0; const ScanStats& ss = s.ss;
+    // ---- per-read segment counting (countRead, depth.d:661-669) for the window / region front ends
+    if (h->seg.on && h->seg.n && ss.n_pass) {
+        if (h->minq) BD_LAUNCH((unsigned)((R + 127) / 128), 128, 0, sm, k_read_segments<true>)(soa, u0, (uint32_t)R, h->seg.s.as<uint64_t>(), h->seg.e.as<uint64_t>(), h->seg.pmax.as<uint64_t>(), h->seg.id.as<uint32_t>(), h->seg.has_min ? h->seg.minstart.as<uint64_t>() : nullptr, h->seg.n, h->seg.reads.as<uint32_t>(), h->minq, h->S, h->seg.has_min ? h->seg.bases_reads.as<uint32_t>() : nullptr);
+        else BD_LAUNCH((unsigned)((R + 127) / 128), 128, 0, sm, k_read_segments<false>)(soa, u0, (uint32_t)R, h->seg.s.as<uint64_t>(), h->seg.e.as<uint64_t>(), h->seg.pmax.as<uint64_t>(), h->seg.id.as<uint32_t>(), h->seg.has_min ? h->seg.minstart.as<uint64_t>() : nullptr, h->seg.n, h->seg.reads.as<uint32_t>(), 0, h->S, h->seg.has_min ? h->seg.bases_reads.as<uint32_t>() : nullptr);
+        CK(cudaGetLastError()); st.gpu_launches++;
+    }
+    uint64_t idx_tiles_base = 0; uint32_t idx_n_tiles = 0;      // K3's per-tile read index of this sub-batch (the mate kernels look reads up through it)
+    // ---- K3
+    uint64_t gmin = std::min<uint64_t>(ss.min_start, ss.min_start_all), gmax = ss.max_end;
+    if (ss.n_zone_pass && gmin < h->cnt_base) gmin = h->cnt_base;      // a zone read may begin before the window; only what reaches this rank's positions matters
+    // (a sub-batch of the zone's first blocks can hold nothing but reads that end before this rank's first position -- the linear index
+    // points at the first read that overlaps the 16 kbp window, the short reads behind it need not: nothing to count then)
+    if ((ss.n_pass || ss.n_zone_pass) && gmax > gmin) {
+        if (gmin < h->cnt_base || gmax > h->cnt_base + h->win_len) {
+            // the index does not describe this file (the reference only checks that one exists, depth.d:1166):
+            // start over with the whole genome as the counter window
+            if (!h->bai_window_ok) return fail(h, BDEPTH_ERR_FORMAT, "read extends past the end of the reference space");
+            h->bai_window_ok = false; CK(cudaDeviceSynchronize());
+            return (h->force_window || h->accum) ? RC_RETRY_WINDOW : RC_RESTART;      // several inputs: the caller starts over with the whole genome as the window
+        }
+        uint64_t t_lo = (gmin - h->cnt_base) / TILE_POS, t_hi = (gmax - h->cnt_base + TILE_POS - 1) / TILE_POS;
+        uint64_t n_tiles = t_hi - t_lo; uint64_t tiles_base = h->cnt_base + t_lo * TILE_POS;
+        idx_tiles_base = tiles_base; idx_n_tiles = (uint32_t)n_tiles;
+        if (t_hi * TILE_POS > h->win_len) return fail(h, BDEPTH_ERR_FORMAT, "read extends past the end of the reference space");
+        CK(h->tile_first.ensure((n_tiles + 2) * 4)); CK(h->tile_lo.ensure((n_tiles + 2) * 4));
+        BD_LAUNCH((unsigned)((n_tiles + 2 + 255) / 256), 256, 0, sm, k_fill_u32)(h->tile_first.as<uint32_t>(), (uint32_t)R, n_tiles + 2);
+        CK(cudaMemsetAsync(h->tile_lo.p, 0xFF, (n_tiles + 2) * 4, sm));
+        if (h->want_presence) { BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_presence)(soa, (uint32_t)R, h->cnt_base, h->win_len, h->present.as<uint32_t>()); st.gpu_launches++; }
+        BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k3_tile_index)(soa, (uint32_t)R, tiles_base, (uint32_t)n_tiles, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>());
+        CK(cudaGetLastError()); st.gpu_launches += 2;
+        for (uint32_t si = 0; si < h->S; si++) {      // one counter set per sample (one pass when combined / single sample)
+            uint32_t* cnt = h->counts.as<uint32_t>() + (uint64_t)si * N_PLANES * h->win_len; int sel = h->S > 1 ? (int)si : -1;
+            if (ss.n_long) {
+                if (h->minq) BD_LAUNCH((unsigned)((ss.n_long * 32 + 255) / 256), 256, 0, sm, k3_scatter_long<true>)(soa, u0, h->long_list.as<uint32_t>(), (uint32_t)ss.n_long, h->cnt_base, h->win_len, cnt, h->minq, sel);
+                else BD_LAUNCH((unsigned)((ss.n_long * 32 + 255) / 256), 256, 0, sm, k3_scatter_long<false>)(soa, u0, h->long_list.as<uint32_t>(), (uint32_t)ss.n_long, h->cnt_base, h->win_len, cnt, 0, sel);
+                CK(cudaGetLastError()); st.gpu_launches++;
+            }
+            if (h->k3_tile) {      // CTA per tile, shared-memory counters, records staged by cp.async.bulk
+                if (h->minq) BD_LAUNCH((unsigned)n_tiles, 256, K3T_SMEM, sm, k3_tile<true>)(soa, u0, (int64_t)s.ub, (uint32_t)R, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, h->minq, sel);
+                else BD_LAUNCH((unsigned)n_tiles, 256, K3T_SMEM, sm, k3_tile<false>)(soa, u0, (int64_t)s.ub, (uint32_t)R, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, 0, sel);
+            } else if (h->k3_pre) {       // round-1 gather kernel with lane-parallel record prefetch (BDEPTH_K3=gather)
+                if (h->minq) BD_LAUNCH((unsigned)n_tiles, 256, 0, sm, k3_gather<true, true>)(soa, u0, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, h->minq, sel);
+                else BD_LAUNCH((unsigned)n_tiles, 256, 0, sm, k3_gather<false, true>)(soa, u0, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, 0, sel);
+            } else if (h->minq) BD_LAUNCH((unsigned)n_tiles, 256, 0, sm, k3_gather<true, false>)(soa, u0, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, h->minq, sel);
+            else BD_LAUNCH((unsigned)n_tiles, 256, 0, sm, k3_gather<false, false>)(soa, u0, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, 0, sel);
+            CK(cudaGetLastError()); st.gpu_launches++;
+        }
+    }
+    // ---- -m: take the worse mate of every overlapping pair out again (mates.cuh)
+    if (fix) {      // where the next batch's stream begins if nothing is open: the first record this batch did not consume
+        const uint64_t tail_abs = batch_u0 + (uint64_t)s.tail; size_t lo = 0, hi = B.size(); while (lo + 1 < hi) { size_t m2 = (lo + hi) / 2; if (B[m2].uoff <= tail_abs) lo = m2; else hi = m2; }
+        P.ghost_b = lo; P.ghost_entry = (int64_t)(tail_abs - B[lo].uoff); P.ghost_below_abs = tail_abs;
+    }
+    if (fix && R && (ss.n_pass || ss.n_ghost || ss.n_ghost_right)) {
+        if (n_subs != 1) return fail(h, BDEPTH_ERR_ARG, "internal: fix-mate-overlaps scans a batch as a whole");
+        uint64_t s_last = 0;       // start of the batch's last record: nothing that follows starts before it
+        CK(cudaMemcpyAsync(&s_last, soa.start + (R - 1), 8, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
+        cudaEvent_t em0 = h->ev[20], em1 = h->ev[21];
+        CK(cudaEventRecord(em0, sm));
+        CK(h->m_hash.ensure((R ? R : 1) * 8)); CK(h->m_flag.ensure((R ? R : 1) * 4)); CK(h->m_ctl.ensure(64));
+        CK(cudaMemsetAsync(h->m_ctl.p, 0, 64, sm)); CK(cudaMemsetAsync((uint8_t*)h->m_ctl.p + 48, 0xFF, 16, sm));       // err, stat; open_off = open_start = none
+        const bool segm = h->seg.on && h->seg.n; const uint32_t n_flt = P.n_flt;      // -L: the regions in flt_d (upload_regions)
+        MateParams mp{soa.start, soa.span, soa.meta, soa.off, soa.ncl, soa.lseq, u0, (uint32_t)R, h->m_hash.as<uint64_t>(), h->m_flag.as<uint32_t>(),
+                      h->flt_d.as<uint64_t>(), h->flt_d.as<uint64_t>() + n_flt, n_flt, h->counts.as<uint32_t>(), h->cnt_base, h->win_len, h->S, h->minq,
+                      segm ? h->seg.s.as<uint64_t>() : nullptr, segm ? h->seg.e.as<uint64_t>() : nullptr, segm ? h->seg.pmax.as<uint64_t>() : nullptr, segm ? h->seg.id.as<uint32_t>() : nullptr,
+                      segm ? h->seg.n : 0u, segm ? h->seg.reads.as<uint32_t>() : nullptr, segm ? h->seg.mbases.as<uint32_t>() : nullptr, h->S,
+                      segm && h->seg.has_u ? h->seg.ustart.as<uint64_t>() : nullptr, segm && h->seg.has_u && h->seg.has_min ? h->seg.minstart.as<uint64_t>() : nullptr, segm && h->seg.has_u ? h->seg.ext_max : 0ull,
+                      h->tile_lo.as<uint32_t>(), idx_tiles_base, idx_n_tiles, h->long_list.as<uint32_t>(), (uint32_t)ss.n_long,
+                      (uint32_t)ss.n_ghost, s_last, P.prev_s_last, P.covered_from, s.last_batch ? 1 : 0, (unsigned long long*)((uint8_t*)h->m_ctl.p + 48), (unsigned long long*)((uint8_t*)h->m_ctl.p + 56),
+                      (s.last_batch && P.blk_hi < B.size()) ? 1 : 0, (unsigned long long*)((uint8_t*)h->m_ctl.p + 40), (uint32_t)ss.n_ghost_right, s.ghost_below == INT64_MIN ? INT64_MIN : s.ghost_below + 4, 0,
+                      (int*)h->m_ctl.p, (unsigned long long*)((uint8_t*)h->m_ctl.p + 16)};
+        const unsigned mg = (unsigned)((R + 127) / 128);
+        BD_LAUNCH(mg, 128, 0, sm, km_hash)(mp); BD_LAUNCH(mg, 128, 0, sm, km_link)(mp); BD_LAUNCH(mg, 128, 0, sm, km_fix)(mp);
+        if (!s.last_batch) { BD_LAUNCH(mg, 128, 0, sm, km_cover)(mp); st.gpu_launches++; }
+        CK(cudaGetLastError()); st.gpu_launches += 3;
+        CK(cudaEventRecord(em1, sm));
+        struct { int err[4]; unsigned long long stat[3]; unsigned long long fix_max_end; unsigned long long open_off, open_start; } ctl;
+        CK(cudaMemcpyAsync(&ctl, h->m_ctl.p, sizeof ctl, cudaMemcpyDeviceToHost, sm));
+        CK(cudaStreamSynchronize(sm));
+        if (ctl.err[0] == MATE_ERR_TOO_MANY) return fail(h, BDEPTH_ERR_ARG, "fix-mate-overlaps: more than %d reads of one name cover one position (record #%d of the batch)", MATE_MAX_MEMBERS, ctl.err[1]);
+        if (ctl.err[0] == MATE_ERR_CROSS) return fail(h, BDEPTH_ERR_ARG, "fix-mate-overlaps: four or more overlapping reads of one name next to a batch boundary (record #%d of the batch): not reproduced there, use larger batches", ctl.err[1]);
+        st.mate_pairs += ctl.stat[0]; st.mate_pair_columns += ctl.stat[1]; st.mate_groups += ctl.stat[2];
+        if (!s.last_batch && ctl.open_off != ~0ull && batch_u0 + (ctl.open_off - 4) < P.ghost_below_abs) {      // something is still open: re-read from its first record
+            const uint64_t g_abs = batch_u0 + (ctl.open_off - 4); size_t lo = 0, hi = B.size(); while (lo + 1 < hi) { size_t m2 = (lo + hi) / 2; if (B[m2].uoff <= g_abs) lo = m2; else hi = m2; }
+            P.ghost_b = lo; P.ghost_entry = (int64_t)(g_abs - B[lo].uoff);
+        }
+        if (ctl.err[0] == MATE_ERR_ZONE) return fail(h, BDEPTH_ERR_ARG, "fix-mate-overlaps on several ranks: overlapping reads of one name reach more than %u BGZF blocks past a shard boundary (record #%d of the batch)", MATE_ZONE_BLOCKS, ctl.err[1]);
+        if (ctl.fix_max_end > P.shard_max && P.shard_min != UINT64_MAX) P.shard_max = ctl.fix_max_end;      // the halo exchange carries the corrections to their owners
+        P.prev_s_last = s_last; P.covered_from = ctl.open_start;
+        { float t = 0; CK(cudaEventElapsedTime(&t, em0, em1)); st.ms_mates += t; }
+    }
+    CK(cudaEventRecord(h->ev[4], sm));
+    // Progressive delivery: positions below the start of the sub-batch's last own read are final (the file is coordinate sorted).  Several ranks
+    // (plain shards): a rank's own positions begin at its first passing read -- known once such a read has been seen -- and the reads of the
+    // previous ranks that reach into them come first in its stream (the zone), so the same holds; where its positions end it learns at the end.
+    Emitter* em = P.em;
+    const bool zone_mode = h->world > 1 && h->comm && !fix && !P.sparse;
+    if (em && zone_mode && h->rank > 0 && P.shard_min != UINT64_MAX) em->lo_clip = P.shard_min;
+    if (em && (h->world == 1 || (zone_mode && (h->rank == 0 || P.shard_min != UINT64_MAX))) && !fix && !s.last_batch && ss.n_pass) { int rce = em->advance(ss.max_start / TILE_POS * TILE_POS, h->ev[4]); if (rce) return rce; }
+    return 0;
+}
+// flagstat / view -c: the records into the counters; the previous rank's zone is that rank's (a sparse view run has none, flagstat is never sparse).
+int consume_census(Pipe& P, const SubBatch& s, bool flagstat) {
+    bdepth* h = P.h; cudaStream_t sm = h->s_main; const uint64_t R = s.R;
+    CK(cudaEventRecord(h->ev[4], sm)); if (!R) return 0;
+    const int64_t own_from = (h->world > 1 && (flagstat || !P.sparse)) ? (int64_t)h->own_lo_abs_u - (int64_t)s.batch_u0 : INT64_MIN;
+    CK(cudaEventRecord(h->ev[22], sm));
+    if (flagstat) BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_flagstat)(s.soa, s.u0, (uint32_t)R, own_from, h->fs.as<unsigned long long>());
+    else BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_view_count)(s.soa, s.u0, (uint32_t)R, own_from, h->vsel, h->vc.as<unsigned long long>());
+    CK(cudaGetLastError()); h->st.gpu_launches++;
+    CK(cudaEventRecord(h->ev[23], sm));
+    P.census_timed = true;
+    return 0;
+}
+// view: the SAM lines of the sub-batch's selected records, handed out before the inflate buffer is reused
+int consume_view_text(Pipe& P, const SubBatch& s) {
+    bdepth* h = P.h; CK(cudaEventRecord(h->ev[4], h->s_main));
+    return s.R ? view_text_sub(h, s.soa, s.u0, (uint32_t)s.R, (h->world > 1 && !P.sparse) ? (int64_t)h->own_lo_abs_u - (int64_t)s.batch_u0 : INT64_MIN) : 0;
+}
+int refuse_index_after_text(bdepth* h) { return fail(h, BDEPTH_ERR_FORMAT, "%s, found after SAM lines were delivered", MSG_CHUNK_MISMATCH); }
+
+// The pipeline: leaves the per-position counters of the whole shard in h->counts (RUN_FULL).
 int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
-    h->coll_pending = 0;
+    h->coll_pending = Owed::NOTHING;
     int rc = init_device(h); if (rc) return rc;
     auto t_host0 = std::chrono::steady_clock::now();
-    bdepth_stats& st = h->st; uint32_t launches0 = 0;
-    st = bdepth_stats{}; st.gpu_launches = launches0;
-    const bool view = mode == RUN_VIEW_COUNT || mode == RUN_VIEW_TEXT;      // view's selection: its count, or its SAM lines
-    if (mode == RUN_VIEW_TEXT) { h->vt.issued = 0; h->vt.ms_fmt = h->vt.ms_d2h = 0; }
-    const bool sparse = (mode == RUN_FULL || view) && plan_sparse(h);      // (view: bdepth_run_view_count / _text has put its own regions there)
-    h->coll_pending = (mode == RUN_FULL && h->world > 1 && h->comm) ? (sparse ? 2 : 1) : (mode == RUN_FLAGSTAT && h->world > 1 && h->comm) ? 3 : (view && h->world > 1 && h->comm) ? (sparse ? 2 : 4) : 0;
+    bdepth_stats& st = h->st; st = bdepth_stats{};
+    const ModeNeeds& need = MODE_NEEDS[mode]; Pipe P{h, mode, ro, em};
+    h->vt.issued = 0; h->vt.ms_fmt = h->vt.ms_d2h = 0;      // every mode: a sparse restart below refuses a run that has handed out SAM lines (vt.issued)
+    const bool sparse = P.sparse = need.may_stage_sparse && plan_sparse(h);      // (view: bdepth_run_view_count / _text has put its own regions there)
+    h->coll_pending = (h->world <= 1 || !h->comm || need.owes == Owed::NOTHING) ? Owed::NOTHING : sparse ? Owed::SPARSE_DECISION : need.owes;      // a sparse query first owes the decision
     if (!sparse) { rc = prepare_shard(h); if (rc) return rc; }      // the plain path needs the whole file's member table (a lazily opened handle frames it now)
     // -m pairs reads of one name wherever they sit in the shard.  A batch is scanned as a whole (no sub-batches), and every
     // batch after the first re-reads the end of the previous one as "ghost" records -- from the earliest record that can
     // still meet a mate (mates.cuh) -- so that a pair cut by a batch boundary is seen complete by the batch that closes it.
-    const bool fix = mode == RUN_FULL && h->fix_mates;
-    bool flt_uploaded = false;            // -L regions on the device for k_ref_seen (once per run)
+    const bool fix = P.fix = mode == RUN_FULL && h->fix_mates;
     if (fix && h->world > 1 && !h->comm) return fail(h, BDEPTH_ERR_ARG, "fix-mate-overlaps on several ranks needs the boundary exchange (bdepth_set_shard with a NCCL id)");
     const uint64_t eff_batch_u = h->batch_u;
-    size_t ghost_b = 0; int64_t ghost_entry = 0; uint64_t ghost_below_abs = 0, prev_s_last = 0, covered_from = 0;      // -m: where the next batch's stream begins
-    const std::vector<HostBlock>& B = sparse ? h->vblocks : h->blocks;
-    const size_t blk_lo = sparse ? 0 : h->blk_lo, blk_hi = sparse ? B.size() : h->blk_hi;
-    const size_t nref = h->hdr.ref_len.size();
+    const std::vector<HostBlock>& B = *(P.B = sparse ? &h->vblocks : &h->blocks);
+    const size_t blk_lo = P.blk_lo = sparse ? 0 : h->blk_lo, blk_hi = P.blk_hi = sparse ? B.size() : h->blk_hi;
     cudaStream_t sm = h->s_main;
 
-    // ---- counter window (28 B/position).  With a BAI the linear index bounds where reads can lie, so only that
-    // span of the linear genome is allocated; without one the whole genome is (87 GB for GRCh38: more than an 80 GB H100 holds, so
-    // such a run ends with the BDEPTH_ERR_CUDA below instead of starting).
-    if (mode == RUN_FULL && h->accum) {
-        // a further input of the same run: counters, window, sample planes stay as the first input left them
-    } else if (mode == RUN_FULL) {
-        uint64_t lo = 0, hi = h->hdr.total_len;
-        if (h->force_window) { lo = h->cnt_base; hi = h->cnt_base + h->win_len; }
-        else
-        if (h->bai.valid && h->bai_window_ok && h->bai.ioffsets.size() == nref && h->world > 1 && !sparse && !fix && blk_hi > blk_lo) {
-            // a shard: from the window in which its first record begins (its own positions begin there or later) to the end of the last
-            // 16 kbp window that any read before the shard's end overlaps (the linear index holds, per window, the first such read)
-            const uint64_t vo_end = blk_hi < B.size() ? (B[blk_hi].coff << 16) : (h->file_len << 16);
-            lo = h->rank == 0 ? UINT64_MAX : h->zone_lin_lo; hi = 0;
-            for (size_t r = 0; r < nref; r++) {
-                const auto& v = h->bai.ioffsets[r];
-                for (size_t k = 0; k < v.size(); k++) if (v[k] && v[k] < vo_end) {
-                    const uint64_t a = h->hdr.ref_lin0[r] + std::min<uint64_t>((uint64_t)k << 14, h->hdr.ref_len[r]), e = h->hdr.ref_lin0[r] + std::min<uint64_t>((uint64_t)(k + 1) << 14, h->hdr.ref_len[r]);
-                    if (h->rank == 0) lo = std::min(lo, a);
-                    if (e > hi) hi = e;
-                }
-            }
-            if (lo == UINT64_MAX || lo >= hi) { lo = 0; hi = h->hdr.total_len; }
-        } else if (h->bai.valid && h->bai_window_ok && h->bai.ioffsets.size() == nref && h->world == 1) {
-            lo = UINT64_MAX; hi = 0;
-            for (size_t r = 0; r < nref; r++) {
-                const auto& v = h->bai.ioffsets[r]; if (v.empty()) continue;
-                size_t k = 0; while (k < v.size() && v[k] == 0) k++;
-                if (k == v.size()) continue;
-                lo = std::min<uint64_t>(lo, h->hdr.ref_lin0[r] + std::min<uint64_t>((uint64_t)k << 14, h->hdr.ref_len[r]));
-                hi = std::max<uint64_t>(hi, h->hdr.ref_lin0[r] + std::min<uint64_t>((uint64_t)v.size() << 14, h->hdr.ref_len[r]));
-            }
-            if (lo >= hi) { lo = 0; hi = h->hdr.total_len; }      // an index without linear entries says nothing
-        }
-        if (!h->force_window) {
-            h->cnt_base = lo / TILE_POS * TILE_POS;
-            h->win_len = ((hi - h->cnt_base + TILE_POS - 1) / TILE_POS + 1) * TILE_POS;
-        }
-        h->S = (h->combined || h->hdr.sample_names.size() <= 1) ? 1u : (uint32_t)h->hdr.sample_names.size();
-        if (h->S > 64) return fail(h, BDEPTH_ERR_ARG, "%u samples: per-sample output supports at most 64 (use --combined)", h->S);
-        size_t need = (size_t)h->win_len * N_PLANES * 4 * h->S;
-        size_t free_b = 0, tot_b = 0; CK(cudaMemGetInfo(&free_b, &tot_b));
-        if (need > h->counts.cap && need > free_b + h->counts.cap) return fail(h, BDEPTH_ERR_CUDA, "counter window needs %zu bytes of HBM, %zu free", need, free_b);
-        CK(h->counts.ensure(need));
-        CK(cudaMemsetAsync(h->counts.p, 0, need, sm));
-        if (h->want_presence) { CK(h->present.ensure((h->win_len / 32 + 2) * 4)); CK(cudaMemsetAsync(h->present.p, 0, (h->win_len / 32 + 2) * 4, sm)); }
-        CK(h->ref_has.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has.p, 0, (nref / 32 + 2) * 4, sm));
-    }
+    if (mode == RUN_FULL) { rc = setup_counter_window(P); if (!rc) rc = upload_rg_table(P); if (!rc) rc = upload_regions(P); if (rc) return rc; }
     CK(h->scan_stats.ensure(sizeof(ScanStats)));
-    const FilterProg* d_fprog = nullptr;
-    if (h->has_fprog && mode != RUN_FLAGSTAT && !view) { CK(h->fprog_d.ensure(sizeof(FilterProg))); CK(cudaMemcpyAsync(h->fprog_d.p, &h->fprog, sizeof(FilterProg), cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm)); d_fprog = h->fprog_d.as<FilterProg>(); }
-    RgTable rgt{nullptr, nullptr, nullptr, 0};
-    if (mode == RUN_FULL && (h->S > 1 || (fix && h->hdr.sample_names.size() > 1))) {      // @RG ID -> sample table for the per-read RG lookup (depth.d:240-250); mates pair within a sample
-        std::vector<uint8_t> ids; std::vector<uint32_t> offs; std::vector<uint8_t> samp;
-        for (size_t g = 0; g < h->hdr.rg_ids.size(); g++) { offs.push_back((uint32_t)ids.size()); ids.insert(ids.end(), h->hdr.rg_ids[g].begin(), h->hdr.rg_ids[g].end()); ids.push_back(0); samp.push_back((uint8_t)h->hdr.rg_sample[g]); }
-        CK(h->rg_ids.ensure(ids.size() + 8)); CK(h->rg_offs.ensure(offs.size() * 4 + 8)); CK(h->rg_samp.ensure(samp.size() + 8));
-        CK(cudaMemcpyAsync(h->rg_ids.p, ids.data(), ids.size(), cudaMemcpyHostToDevice, sm)); CK(cudaMemcpyAsync(h->rg_offs.p, offs.data(), offs.size() * 4, cudaMemcpyHostToDevice, sm)); CK(cudaMemcpyAsync(h->rg_samp.p, samp.data(), samp.size(), cudaMemcpyHostToDevice, sm));
-        CK(cudaStreamSynchronize(sm));
-        rgt = RgTable{h->rg_ids.as<uint8_t>(), h->rg_offs.as<uint32_t>(), h->rg_samp.as<uint8_t>(), (uint32_t)offs.size()};
-    }
+    if (h->has_fprog && need.loads_fprog) { CK(h->fprog_d.ensure(sizeof(FilterProg))); CK(cudaMemcpyAsync(h->fprog_d.p, &h->fprog, sizeof(FilterProg), cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm)); P.d_fprog = h->fprog_d.as<FilterProg>(); }
     { uint64_t shard_u = blk_hi > blk_lo ? B[blk_hi - 1].uoff + B[blk_hi - 1].isize - B[blk_lo].uoff : 0; CK(h->ubuf.ensure(CARRY_MAX + std::min<uint64_t>(eff_batch_u + 65536, shard_u) + 256)); }
     CK(h->misc.ensure(64));
     HostScratch& hs = h->hs;
-    // up(): host words -> device buffer; down(): device words -> mapped host memory, readable after the next
-    // synchronisation of the main stream.  Both are stream-ordered kernels on the main stream.
-    auto up = [&](void* dst_dev, const void* src, size_t bytes) -> int {
-        if (!bytes) return 0;
-        uint8_t* m = hs.take(bytes); if (!m) return fail(h, BDEPTH_ERR_CUDA, "internal: host scratch exhausted");
-        memcpy(m, src, bytes);
-        BD_LAUNCH((unsigned)std::min<size_t>((bytes / 4 + 255) / 256, 512), 256, 0, sm, k_copy_words)((uint32_t*)dst_dev, (const uint32_t*)hs.dev(m), bytes / 4);
-        st.gpu_launches++;
-        return 0;
-    };
-    auto down = [&](const void* src_dev, size_t bytes) -> uint8_t* {
-        uint8_t* m = hs.take(bytes ? bytes : 4); if (!m) return nullptr;
-        if (bytes) { BD_LAUNCH((unsigned)std::min<size_t>((bytes / 4 + 255) / 256, 512), 256, 0, sm, k_copy_words)((uint32_t*)hs.dev(m), (const uint32_t*)src_dev, bytes / 4); st.gpu_launches++; }
-        return m;
-    };
-#define UP(dst, src, bytes) do { int rcu_ = up((dst), (src), (bytes)); if (rcu_) return rcu_; } while (0)
-#define DOWN(var, type, src, bytes) type* var = (type*)down((src), (bytes)); if (!var) return fail(h, BDEPTH_ERR_CUDA, "internal: host scratch exhausted")
-
     float ms_h2d = 0, ms_k1 = 0, ms_k2 = 0, ms_k3 = 0;
-    uint64_t carry_len = 0; bool first_batch = true;
     bool sparse_bad = false;         // a region chunk's record chain did not end at the chunk end (several ranks: decided together after the batches)
-    uint64_t shard_min = UINT64_MAX, shard_max = 0;
-    if (mode == RUN_INDEX) {      // tables of k_index_scan: one linear-index row per reference (16 kbp windows up to one past the reference end), counters, carry
-        auto& X = h->ix; X.base.assign(nref + 1, 0); X.cap.assign(nref + 1, 0); uint64_t acc = 0;
-        for (size_t r = 0; r < nref; r++) { X.base[r] = (uint32_t)acc; X.cap[r] = (uint32_t)std::min<uint64_t>(32769, ((uint64_t)h->hdr.ref_len[r] >> 14) + 2); acc += X.cap[r]; if (acc > 0xFFFFFFF0ull) return fail(h, BDEPTH_ERR_ARG, "too many references for the linear index tables"); }
-        X.n_lin = acc; X.h_runs.clear(); X.h_excs.clear();
-        CK(X.lin.ensure((acc + 1) * 8)); CK(X.lin_len.ensure((nref + 1) * 4)); CK(X.lin_base.ensure((nref + 1) * 4)); CK(X.lin_cap.ensure((nref + 1) * 4));
-        CK(X.n_mapped.ensure((nref + 1) * 8)); CK(X.n_unmapped.ensure((nref + 1) * 8)); CK(X.carry.ensure(sizeof(IndexCarry))); CK(X.ctl.ensure(sizeof(IndexCtl)));
-        CK(cudaMemsetAsync(X.lin.p, 0xFF, (acc + 1) * 8, sm)); CK(cudaMemsetAsync(X.lin_len.p, 0, (nref + 1) * 4, sm)); CK(cudaMemsetAsync(X.n_mapped.p, 0, (nref + 1) * 8, sm)); CK(cudaMemsetAsync(X.n_unmapped.p, 0, (nref + 1) * 8, sm));
-        CK(cudaMemsetAsync(X.carry.p, 0, sizeof(IndexCarry), sm));
-        CK(cudaMemcpyAsync(X.lin_base.p, X.base.data(), (nref + 1) * 4, cudaMemcpyHostToDevice, sm)); CK(cudaMemcpyAsync(X.lin_cap.p, X.cap.data(), (nref + 1) * 4, cudaMemcpyHostToDevice, sm));
-        IndexCtl c0{0, 0, 0, ~0ull, ~0ull, 0, ~0ull, 0};
-        CK(cudaMemcpyAsync(X.ctl.p, &c0, sizeof c0, cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm));
+    switch (mode) {      // the consumer's tables and counters (depth's were set up above)
+        case RUN_INDEX: rc = setup_index_tables(h); if (rc) return rc; break;
+        case RUN_FLAGSTAT: case RUN_VIEW_COUNT: case RUN_VIEW_TEXT: { const Census c = census_of(h, need.owes); CK(c.d.ensure(c.words * 8)); CK(cudaMemsetAsync(c.d.p, 0, c.words * 8, sm)); break; }
+        default: break;
     }
-    float ms_census = 0;
-    if (mode == RUN_FLAGSTAT) { CK(h->fs.ensure((FS_WORDS + 1) * 8)); CK(cudaMemsetAsync(h->fs.p, 0, (FS_WORDS + 1) * 8, sm)); }
-    if (view) { CK(h->vc.ensure(16)); CK(cudaMemsetAsync(h->vc.p, 0, 16, sm)); }
     CK(cudaEventRecord(h->ev[10], sm));
     size_t b = blk_lo;
     if (ro) { ro->inflate_len = 0; ro->scan_n = 0; }
-    if (!h->staged) {   // size both compressed-data buffers for the largest batch up front (ensure() must not reallocate mid-flight)
-        uint64_t mx = 0;
-        for (size_t bb = blk_lo; bb < blk_hi;) {
-            size_t e = bb; uint64_t u = 0, cb = 0; while (e < blk_hi && (e == bb || u + B[e].isize <= eff_batch_u)) { u += B[e].isize; cb += B[e].bsize; e++; }
-            mx = std::max<uint64_t>(mx, sparse ? cb + 8 : B[e - 1].coff + B[e - 1].bsize - (B[bb].coff & ~3ull)); bb = e;
-        }
-        CK(h->comp2[0].ensure(mx + 256)); CK(h->comp2[1].ensure(mx + 256));
-    }
     size_t batch_no = 0;
     auto batch_end = [&](size_t bb) { size_t e = bb; uint64_t u = 0; while (e < blk_hi && (e == bb || u + B[e].isize <= eff_batch_u)) { u += B[e].isize; e++; } return e; };
-    // H2D of blocks [bb, be) into comp2[slot]; waits until K1 of the batch that used the slot two batches ago is done
-    const size_t H2D_CHUNK_BLOCKS = h->chunk_blocks;
-    // dco[slot][i] = where block bb+i of the batch sits in comp2[slot].  Plain runs keep the file layout (one copy
-    // per chunk); sparse runs pack the selected blocks back to back (one copy per run of file-adjacent blocks).
-    std::vector<uint64_t> dco[2];
-    auto issue_h2d = [&](size_t no, size_t bb, size_t be) -> int {
-        int slot = (int)(no & 1);
-        uint64_t g0 = B[bb].coff & ~3ull;
-        if (no >= 2) CK(cudaStreamWaitEvent(h->s_copy, h->ev[16 + slot], 0));
-        CK(cudaEventRecord(h->ev[18 + slot], h->s_copy));
-        h->chunk_end[slot].clear();
-        dco[slot].resize(be - bb);
-        { uint64_t acc = 0; for (size_t i = bb; i < be; i++) { dco[slot][i - bb] = sparse ? acc : B[i].coff - g0; acc += B[i].bsize; } }
-        size_t nch = 0;
-        for (size_t c0 = bb; c0 < be; c0 += H2D_CHUNK_BLOCKS, nch++) {
-            size_t c1 = std::min(be, c0 + H2D_CHUNK_BLOCKS);
-            uint64_t dev_end;
-            if (!sparse) {
-                uint64_t a = c0 == bb ? g0 : B[c0].coff, e = B[c1 - 1].coff + B[c1 - 1].bsize;
-                CK(cudaMemcpyAsync((uint8_t*)h->comp2[slot].p + (a - g0), h->file + a, e - a, cudaMemcpyHostToDevice, h->s_copy));
-                dev_end = e - g0;
-            } else {
-                for (size_t r0 = c0; r0 < c1;) {
-                    size_t r1 = r0 + 1; while (r1 < c1 && B[r1].coff == B[r1 - 1].coff + B[r1 - 1].bsize) r1++;
-                    CK(cudaMemcpyAsync((uint8_t*)h->comp2[slot].p + dco[slot][r0 - bb], h->file + B[r0].coff, B[r1 - 1].coff + B[r1 - 1].bsize - B[r0].coff, cudaMemcpyHostToDevice, h->s_copy));
-                    r0 = r1;
-                }
-                dev_end = dco[slot][c1 - 1 - bb] + B[c1 - 1].bsize;
-            }
-            if (c1 == be) CK(cudaMemsetAsync((uint8_t*)h->comp2[slot].p + dev_end, 0, 128, h->s_copy));
-            if (h->chunk_ev[slot].size() <= nch) { cudaEvent_t ne; CK(cudaEventCreateWithFlags(&ne, cudaEventDisableTiming)); h->chunk_ev[slot].push_back(ne); }
-            CK(cudaEventRecord(h->chunk_ev[slot][nch], h->s_copy));
-            h->chunk_end[slot].push_back(c1);
-        }
-        CK(cudaEventRecord(h->ev[14 + slot], h->s_copy));
-        return 0;
-    };
+    auto comp_bytes = [&](size_t bb, size_t e) { uint64_t n = 8; if (sparse) for (size_t i = bb; i < e; i++) n += B[i].bsize; else n = B[e - 1].coff + B[e - 1].bsize - (B[bb].coff & ~3ull); return n; };
+    if (!h->staged) {   // size both compressed-data buffers for the largest batch up front (ensure() must not reallocate mid-flight)
+        uint64_t mx = 0; for (size_t bb = blk_lo; bb < blk_hi; bb = batch_end(bb)) mx = std::max<uint64_t>(mx, comp_bytes(bb, batch_end(bb)));
+        CK(h->comp2[0].ensure(mx + 256)); CK(h->comp2[1].ensure(mx + 256));
+    }
     while (b < blk_hi) {
         // ---- batch extent
-        size_t b1 = b; uint64_t ub_new = 0;
-        while (b1 < blk_hi && (b1 == b || ub_new + B[b1].isize <= eff_batch_u)) { ub_new += B[b1].isize; b1++; }
+        const size_t b1 = batch_end(b);
         const bool last_batch = b1 == blk_hi;
-        st.n_batches++; st.n_blocks += b1 - b; st.inflated_bytes += ub_new;
+        st.n_batches++; st.n_blocks += b1 - b; for (size_t i = b; i < b1; i++) st.inflated_bytes += B[i].isize;
         const size_t new_b = b;                                                          // first block that has not been scanned yet
-        const size_t stream_b = (fix && batch_no > 0) ? std::min(ghost_b, b) : b;          // -m: the batch's stream begins with re-read blocks
+        const size_t stream_b = (fix && batch_no > 0) ? std::min(P.ghost_b, b) : b;      // -m: the batch's stream begins with re-read blocks
         {   // from here to the end of the sub-batch loop `b` is the first block of the batch's stream
-        const size_t b = stream_b;
-        const size_t nb = b1 - b;
-        const uint64_t batch_u0 = B[b].uoff;               // absolute inflated offset of the batch start
-        const uint64_t ub = B[b1 - 1].uoff + B[b1 - 1].isize - batch_u0;
+        const size_t b = stream_b, nb = b1 - b;
+        const uint64_t batch_u0 = B[b].uoff, ub = B[b1 - 1].uoff + B[b1 - 1].isize - batch_u0;      // absolute inflated offset of the batch start, its bytes
         // ---- compressed bytes on the device: H2D runs on the copy stream into one of two buffers, so the copy of
         // batch i+1 overlaps the kernels of batch i
         const uint32_t* d_comp;
@@ -932,17 +1331,16 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         if (h->staged) d_comp = h->comp.as<uint32_t>();
         else {
             if (fix) {       // no prefetch: where a batch begins is only known when the previous one has been scanned
-                uint64_t need = 8; if (sparse) for (size_t i = b; i < b1; i++) need += B[i].bsize; else need = B[b1 - 1].coff + B[b1 - 1].bsize - (B[b].coff & ~3ull);
-                CK(h->comp2[batch_no & 1].ensure(need + 256));
-                int rcp = issue_h2d(batch_no, b, b1); if (rcp) return rcp;
-            } else if (batch_no == 0) { int rcp = issue_h2d(0, b, b1); if (rcp) return rcp; }
+                CK(h->comp2[batch_no & 1].ensure(comp_bytes(b, b1) + 256));
+                rc = issue_h2d(P, batch_no, b, b1); if (rc) return rc;
+            } else if (batch_no == 0) { rc = issue_h2d(P, 0, b, b1); if (rc) return rc; }
             d_comp = h->comp2[batch_no & 1].as<uint32_t>();
         }
         // ---- descriptors
         std::vector<BlockDesc> d(nb); uint64_t csum = 0, tok_words = 0;
         for (size_t i = 0; i < nb; i++) {
             const HostBlock& hb = B[b + i];
-            uint64_t dev_off = h->staged ? hb.coff - h->staged_file_off : dco[batch_no & 1][i];
+            uint64_t dev_off = h->staged ? hb.coff - h->staged_file_off : P.dco[batch_no & 1][i];
             d[i] = BlockDesc{dev_off + hb.cdata_off, hb.uoff - batch_u0, hb.csize, hb.isize, tok_words};
             tok_words += tok_cap_of(hb.isize);
             if (b + i >= new_b) { csum += hb.csize; st.file_bytes += hb.bsize; }
@@ -952,411 +1350,80 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
         if (!h->k1_onephase) { CK(h->tok.ensure(tok_words * 4 + 64)); CK(h->lits.ensure(ub + 16 * nb + 64)); CK(h->aux.ensure(nb * sizeof(BlockAux))); CK(h->segi.ensure(nb * MAX_SEG * 4)); CK(h->littab.ensure(nb * (size_t)MAX_SEG * 256)); }
         CK(hs.ensure(nb * (sizeof(BlockDesc) + 192) + 16384)); hs.used = 0;      // nothing is in flight here: every sub-batch ends synchronised
         UP(h->descs.p, d.data(), nb * sizeof(BlockDesc));
-        uint8_t* u0 = h->ubuf.as<uint8_t>() + CARRY_MAX;     // offset 0 of this batch's inflated bytes
+        uint8_t* const m_u0 = h->ubuf.as<uint8_t>() + CARRY_MAX;     // offset 0 of this batch's inflated bytes
         CK(cudaEventRecord(e1, sm));
         struct Sub { size_t s0, s1; int ev_lo, ev_hi; };     // blocks [s0, s1) are inflated once k1_ev[ev_lo..ev_hi] have fired
         std::vector<Sub> subs;
         // ---- K1: when the input is streaming in, one sub-launch per H2D chunk, spread over a few streams so that
         // they run side by side (a lone sub-launch cannot fill the GPU: every lane owns a whole BGZF block)
-        // K1 of blocks [c0, c0 + n) of the batch on stream ks: the two-phase inflater (k1_huff, k1_lz) and the exact one-phase kernel
-        // for whatever phase 1 handed back (normally nothing: it returns at once); BDEPTH_K1_ONEPHASE=1 runs the round-1 kernel alone (A/B)
-        auto launch_k1 = [&](cudaStream_t ks, size_t c0, uint32_t n) -> int {
-            const BlockDesc* dd = h->descs.as<BlockDesc>() + (c0 - b); int* stp = h->status.as<int>() + (c0 - b);
-            if (h->k1_onephase) {
-                BD_LAUNCH((n + 32 * K1_WARPS - 1) / (32 * K1_WARPS), 32 * K1_WARPS, K1_SMEM, ks, k1_inflate)(d_comp, dd, n, u0, stp);
-                CK(cudaGetLastError()); st.gpu_launches++;
-                return 0;
-            }
-            BlockAux* ax = h->aux.as<BlockAux>() + (c0 - b); uint32_t* sgi = h->segi.as<uint32_t>() + (c0 - b) * MAX_SEG; uint8_t* ltb = h->littab.as<uint8_t>() + (c0 - b) * (size_t)MAX_SEG * 256;
-            const unsigned hg = (n + 32 * K1H_WARPS - 1) / (32 * K1H_WARPS); const uint32_t blk0 = (uint32_t)(c0 - b);
-#define K1H(LIMS, MINB) BD_LAUNCH(hg, 32 * K1H_WARPS, k1h_smem<LIMS>(), ks, k1_huff<LIMS, MINB>)(d_comp, dd, n, blk0, stp, h->tok.as<uint32_t>(), h->lits.as<uint8_t>(), ax, sgi, ltb)
-            // which instantiation: limits in registers at 4 CTAs per SM (16 warps) is the faster loop; when a launch has more warps than that
-            // holds at once (16 warps on every SM of the device), limits in shared memory at 5 CTAs (20 warps) wins by its occupancy
-            const int variant = h->k1h_variant >= 0 ? h->k1h_variant : (n > (uint32_t)h->n_sm * 16u * 32u ? 2 : 0);
-            switch (variant) { case 1: K1H(false, 6); break; case 2: K1H(true, 5); break; case 3: K1H(true, 4); break; default: K1H(false, 4); }
-#undef K1H
-            if (h->k1lz_flat) BD_LAUNCH((n + K1L_WARPS - 1) / K1L_WARPS, 32 * K1L_WARPS, 0, ks, k1_lz_flat)(dd, n, blk0, u0, stp, h->tok.as<uint32_t>(), h->lits.as<uint8_t>(), ax, sgi, ltb);
-            else if (h->k1lz_v12) BD_LAUNCH((n + K1L_WARPS - 1) / K1L_WARPS, 32 * K1L_WARPS, 0, ks, k1_lz<false>)(dd, n, blk0, u0, stp, h->tok.as<uint32_t>(), h->lits.as<uint8_t>(), ax, sgi, ltb);
-            else BD_LAUNCH((n + K1L_WARPS - 1) / K1L_WARPS, 32 * K1L_WARPS, 0, ks, k1_lz<true>)(dd, n, blk0, u0, stp, h->tok.as<uint32_t>(), h->lits.as<uint8_t>(), ax, sgi, ltb);
-            BD_LAUNCH((n + 32 * K1_WARPS - 1) / (32 * K1_WARPS), 32 * K1_WARPS, K1_SMEM, ks, k1_fallback)(d_comp, dd, n, u0, stp);
-            CK(cudaGetLastError()); st.gpu_launches += 3;
-            return 0;
-        };
         if (h->staged) {
-            { int rck = launch_k1(sm, b, (uint32_t)nb); if (rck) return rck; }
+            rc = launch_k1(h, sm, d_comp, m_u0, b, b, (uint32_t)nb); if (rc) return rc;
             subs.push_back(Sub{b, b1, 0, -1});
         } else {
             int slot = (int)(batch_no & 1); size_t c0 = b;
             for (size_t j = 0; j < h->chunk_end[slot].size(); j++) {
                 size_t c1 = h->chunk_end[slot][j]; cudaStream_t ks = h->s_k1[j & 15];
                 CK(cudaStreamWaitEvent(ks, e1, 0)); CK(cudaStreamWaitEvent(ks, h->chunk_ev[slot][j], 0));
-                uint32_t n = (uint32_t)(c1 - c0);
-                { int rck = launch_k1(ks, c0, n); if (rck) return rck; }
+                rc = launch_k1(h, ks, d_comp, m_u0, b, c0, (uint32_t)(c1 - c0)); if (rc) return rc;
                 if (h->k1_ev.size() <= j) { cudaEvent_t ne; CK(cudaEventCreateWithFlags(&ne, cudaEventDisableTiming)); h->k1_ev.push_back(ne); }
                 CK(cudaEventRecord(h->k1_ev[j], ks));
                 // Sub-batches: a lane needs ~60 ms for its block however empty the GPU is, so the scan / coverage /
                 // delivery of the blocks that arrived first runs while the later chunks are still being inflated.
-                if ((mode == RUN_FULL || mode == RUN_INDEX || mode == RUN_FLAGSTAT || view) && !fix) subs.push_back(Sub{c0, c1, (int)j, (int)j}); else { if (subs.empty()) subs.push_back(Sub{b, b1, 0, (int)j}); subs[0].ev_hi = (int)j; }
+                if (need.sub_batched && !fix) subs.push_back(Sub{c0, c1, (int)j, (int)j}); else { if (subs.empty()) subs.push_back(Sub{b, b1, 0, (int)j}); subs[0].ev_hi = (int)j; }
                 c0 = c1;
             }
         }
-        if (!h->staged && !fix && b1 < blk_hi) { int rcp = issue_h2d(batch_no + 1, b1, batch_end(b1)); if (rcp) return rcp; }
-        const size_t mb = b, mb1 = b1; const uint64_t m_u0abs = batch_u0; uint8_t* const m_u0 = u0; const bool m_last = last_batch;
+        if (!h->staged && !fix && b1 < blk_hi) { rc = issue_h2d(P, batch_no + 1, b1, batch_end(b1)); if (rc) return rc; }
         for (size_t sbi = 0; sbi < subs.size(); sbi++) {
-        const size_t b = subs[sbi].s0, b1 = subs[sbi].s1, nb = b1 - b;                  // from here on: the sub-batch
-        const uint64_t batch_u0 = B[b].uoff, ub = B[b1 - 1].uoff + B[b1 - 1].isize - batch_u0;
-        uint8_t* const u0 = m_u0 + (batch_u0 - m_u0abs);
-        const bool last_sub = sbi + 1 == subs.size(), last_batch = m_last && last_sub;
+        const size_t sb0 = subs[sbi].s0, sb1 = subs[sbi].s1, snb = sb1 - sb0;                  // the sub-batch
+        SubBatch s; s.batch_u0 = B[sb0].uoff; s.ub = B[sb1 - 1].uoff + B[sb1 - 1].isize - s.batch_u0; s.u0 = m_u0 + (s.batch_u0 - batch_u0);
+        s.last_sub = sbi + 1 == subs.size(); s.last_batch = last_batch && s.last_sub; s.batch_no = batch_no;
         for (int j = subs[sbi].ev_lo; j <= subs[sbi].ev_hi; j++) CK(cudaStreamWaitEvent(sm, h->k1_ev[j], 0));
         CK(cudaEventRecord(e2, sm));
-        if (!h->staged && last_sub) CK(cudaEventRecord(h->ev[16 + (batch_no & 1)], sm));     // this batch's compressed buffer is free again
-        DOWN(stt, int, h->status.as<int>() + (b - mb), nb * sizeof(int));
+        if (!h->staged && s.last_sub) CK(cudaEventRecord(h->ev[16 + (batch_no & 1)], sm));     // this batch's compressed buffer is free again
+        DOWN(stt, int, h->status.as<int>() + (sb0 - b), snb * sizeof(int));
         if (mode == RUN_INFLATE_ONLY) {
             CK(cudaStreamSynchronize(sm));
-            for (size_t i = 0; i < nb; i++) if (stt[i]) return fail(h, BDEPTH_ERR_FORMAT, "DEFLATE error %d in BGZF block at offset %llu", stt[i], (unsigned long long)B[b + i].coff);
+            for (size_t i = 0; i < snb; i++) if (stt[i]) return fail(h, BDEPTH_ERR_FORMAT, "DEFLATE error %d in BGZF block at offset %llu", stt[i], (unsigned long long)B[sb0 + i].coff);
             if (ro && ro->inflate_dst) {
-                if (ro->inflate_len + ub > ro->inflate_cap) return fail(h, BDEPTH_ERR_ARG, "inflate buffer too small");
-                CK(cudaMemcpy(ro->inflate_dst + ro->inflate_len, u0, ub, cudaMemcpyDeviceToHost));
+                if (ro->inflate_len + s.ub > ro->inflate_cap) return fail(h, BDEPTH_ERR_ARG, "inflate buffer too small");
+                CK(cudaMemcpy(ro->inflate_dst + ro->inflate_len, s.u0, s.ub, cudaMemcpyDeviceToHost));
             }
-            if (ro) ro->inflate_len += ub;
+            if (ro) ro->inflate_len += s.ub;
             float t; CK(cudaEventElapsedTime(&t, e1, e2)); ms_k1 += t;
             continue;
         }
-        // ---- K2: chunk table
-        const bool seg0 = sparse && h->seg_entry[b] >= 0;      // the sub-batch begins a new region-query chunk: nothing is carried into it
-        if (seg0) carry_len = 0;
-        std::vector<int64_t> cstart(nb + 1); std::vector<uint32_t> sbase(nb + 1);
-        { uint64_t acc = 0; for (size_t i = 0; i < nb; i++) { cstart[i] = (int64_t)(B[b + i].uoff - batch_u0); sbase[i] = (uint32_t)acc; uint64_t sz = B[b + i].isize + (i == 0 ? carry_len : 0); acc += sz / 36 + 2; } cstart[nb] = (int64_t)ub; sbase[nb] = (uint32_t)acc; cstart[0] = -(int64_t)carry_len;
-          if (acc > 0xFFFFFFFFull) return fail(h, BDEPTH_ERR_ARG, "batch too large"); }
-        const uint64_t n_slots = sbase[nb];
-        CK(h->chunk_start.ensure((nb + 1) * 8)); CK(h->slot_base.ensure((nb + 1) * 4)); CK(h->entry.ensure(nb * 8)); CK(h->exitb.ensure(nb * 8)); CK(h->count.ensure(nb * 4)); CK(h->rec_base.ensure((nb + 1) * 4)); CK(h->slots.ensure(n_slots * 2 + 64)); CK(h->walk_list.ensure(64));
-        UP(h->chunk_start.p, cstart.data(), (nb + 1) * 8);
-        UP(h->slot_base.p, sbase.data(), (nb + 1) * 4);
-        CK(cudaMemsetAsync(h->entry.p, ENTRY_NONE_BYTE, nb * 8, sm));
-        // (-m: a stream that begins exactly where a region-query chunk begins starts at that chunk's first record)
-        int64_t anchor = (fix && batch_no > 0) ? ((seg0 && ghost_entry < (int64_t)h->seg_entry[b]) ? (int64_t)h->seg_entry[b] : ghost_entry) : seg0 ? (int64_t)h->seg_entry[b] : first_batch ? h->entry0 : -(int64_t)carry_len;
-        UP(h->entry.p, &anchor, 8);
-        CK(cudaMemsetAsync(h->misc.p, 0, 64, sm));
-        // records that START at or after the shard limit belong to the next rank
-        int64_t u_limit = (int64_t)ub; if (!sparse && h->limit_abs_u < batch_u0 + ub) u_limit = (int64_t)h->limit_abs_u - (int64_t)batch_u0;      // may be negative: the limit lies before this sub-batch, and a carried record that starts at or after it is not ours either
-        ScanParams sp{u0, -(int64_t)carry_len, (int64_t)ub, (int)nref, h->ref_len_d.as<uint32_t>(), h->ref_lin0_d.as<uint64_t>()};
-        BD_LAUNCH((unsigned)((nb * 32 + 255) / 256), 256, 0, sm, k2_guess_entries)(sp, h->chunk_start.as<int64_t>(), (uint32_t)nb, h->entry.as<int64_t>());
-        CK(cudaGetLastError()); st.gpu_launches++;
-        const int64_t* d_limit = nullptr;
-        if (sparse) {       // chunks of the region query: exact entries at their first blocks, walk limits at their last ones
-            std::vector<uint32_t> ai; std::vector<int64_t> av; std::vector<int64_t> lim(nb, INT64_MAX);
-            for (size_t i = 0; i < nb; i++) {
-                if (i && h->seg_entry[b + i] >= 0) { ai.push_back((uint32_t)i); av.push_back(cstart[i] + h->seg_entry[b + i]); }
-                if (h->seg_limit[b + i] != UINT32_MAX) lim[i] = (i ? cstart[i] : 0) + (int64_t)h->seg_limit[b + i];
-            }
-            CK(h->chunk_limit.ensure(nb * 8)); UP(h->chunk_limit.p, lim.data(), nb * 8); d_limit = h->chunk_limit.as<int64_t>();
-            if (!ai.empty()) {
-                CK(h->anchors_idx.ensure(ai.size() * 4)); CK(h->anchors_val.ensure(av.size() * 8));
-                UP(h->anchors_idx.p, ai.data(), ai.size() * 4); UP(h->anchors_val.p, av.data(), av.size() * 8);
-                BD_LAUNCH((unsigned)((ai.size() + 255) / 256), 256, 0, sm, k_scatter_i64)(h->entry.as<int64_t>(), h->anchors_idx.as<uint32_t>(), h->anchors_val.as<int64_t>(), (uint32_t)ai.size());
-                CK(cudaGetLastError()); st.gpu_launches++;
-            }
+        rc = walk_records(P, s, sb0, sb1, stt); if (rc) return rc;
+        if (s.mismatch) {
+            // the index does not describe this file (the reference only checks that one exists): plain pass instead.
+            // On several ranks that decision has to be taken by all of them together (below, after the batches):
+            // a rank falling back on its own would leave the union of the ranks' records no partition of the file.
+            if (h->world == 1) { if (h->vt.issued) return refuse_index_after_text(h); h->sparse_ok = false; CK(cudaDeviceSynchronize()); return RC_RESTART; }
+            sparse_bad = true; break;
         }
-        ScanParams spw = sp;
-        BD_LAUNCH((unsigned)((nb + 127) / 128), 128, 0, sm, k2_walk)(spw, h->chunk_start.as<int64_t>(), (uint32_t)nb, h->entry.as<int64_t>(), h->slot_base.as<uint32_t>(), h->slots.as<uint16_t>(), h->count.as<uint32_t>(), h->exitb.as<int64_t>(), (int*)h->misc.p, nullptr, 0, d_limit);
-        CK(cudaGetLastError()); st.gpu_launches++;
-        DOWN(ent, int64_t, h->entry.p, nb * 8); DOWN(ext, int64_t, h->exitb.p, nb * 8); DOWN(cnt, uint32_t, h->count.p, nb * 4);      // host-owned once synchronised
-        DOWN(werr, int, h->misc.p, 4);
-        CK(cudaStreamSynchronize(sm));
-        int walk_err = *werr;
-        for (size_t i = 0; i < nb; i++) if (stt[i]) return fail(h, BDEPTH_ERR_FORMAT, "DEFLATE error %d in BGZF block at offset %llu", stt[i], (unsigned long long)B[b + i].coff);
-        // ---- exact chain verification (host, control plane): entry[i] must equal the running exit
-        int64_t cur = anchor; int64_t tail = (int64_t)ub;
-        for (size_t i = 0; i < nb; i++) {
-            if (sparse && i && h->seg_entry[b + i] >= 0) cur = cstart[i] + h->seg_entry[b + i];     // a new chunk: the chain restarts at its first record
-            int64_t true_e = (cur < cstart[i + 1]) ? cur : ENTRY_NONE;
-            if (true_e != ENTRY_NONE && true_e < cstart[i]) return fail(h, BDEPTH_ERR_FORMAT, "internal: record chain went backwards");
-            if (ent[i] != true_e) {
-                st.chain_fixups++;
-                uint32_t ci = (uint32_t)i;
-                UP((int64_t*)h->entry.p + i, &true_e, 8);
-                UP(h->walk_list.p, &ci, 4);
-                BD_LAUNCH(1, 32, 0, sm, k2_walk)(spw, h->chunk_start.as<int64_t>(), (uint32_t)nb, h->entry.as<int64_t>(), h->slot_base.as<uint32_t>(), h->slots.as<uint16_t>(), h->count.as<uint32_t>(), h->exitb.as<int64_t>(), (int*)h->misc.p, h->walk_list.as<uint32_t>(), 1, d_limit);
-                CK(cudaGetLastError()); st.gpu_launches++;
-                DOWN(fx_ext, int64_t, (int64_t*)h->exitb.p + i, 8); DOWN(fx_cnt, uint32_t, (uint32_t*)h->count.p + i, 4); DOWN(fx_err, int, h->misc.p, 4);
-                CK(cudaStreamSynchronize(sm));
-                ext[i] = *fx_ext; cnt[i] = *fx_cnt; walk_err = *fx_err;
-                ent[i] = true_e;
-            }
-            if (true_e != ENTRY_NONE) {
-                cur = ext[i];
-                if (sparse && h->seg_limit[b + i] != UINT32_MAX) {      // last block of a chunk: the chain must end exactly at the chunk end
-                    if (ext[i] != (i ? cstart[i] : 0) + (int64_t)h->seg_limit[b + i]) {
-                        // the index does not describe this file (the reference only checks that one exists): plain pass instead.
-                        // On several ranks that decision has to be taken by all of them together (below, after the batches):
-                        // a rank falling back on its own would leave the union of the ranks' records no partition of the file.
-                        if (h->world == 1) { if (mode == RUN_VIEW_TEXT && h->vt.issued) return fail(h, BDEPTH_ERR_FORMAT, "the index does not describe this file (a region chunk does not end at a record), found after SAM lines were delivered"); h->sparse_ok = false; CK(cudaDeviceSynchronize()); return run_pipeline(h, mode, ro, em); }
-                        sparse_bad = true; break;
-                    }
-                    cur = INT64_MAX / 2;                                  // nothing follows until the next chunk begins
-                    continue;
-                }
-                if (ext[i] < cstart[i + 1]) {      // the walk stopped inside its own block: incomplete tail record
-                    for (size_t j = i + 1; j < nb; j++) cnt[j] = 0;
-                    break;
-                }
-            }
+        rc = decode_records(P, s, snb); if (rc) return rc;
+        switch (mode) {
+            case RUN_SCAN_ONLY: rc = consume_scan(P, s); break;
+            case RUN_INDEX: rc = consume_index(P, s); break;
+            case RUN_FULL: rc = consume_depth(P, s, subs.size()); break;
+            case RUN_FLAGSTAT: rc = consume_census(P, s, true); break;
+            case RUN_VIEW_COUNT: rc = consume_census(P, s, false); break;
+            case RUN_VIEW_TEXT: rc = consume_view_text(P, s); break;
+            case RUN_INFLATE_ONLY: break;
         }
-        if (sparse_bad) break;
-        if (walk_err) return fail(h, BDEPTH_ERR_FORMAT, "corrupt BAM record chain (block_size < 32)");
-        tail = cur < (int64_t)ub ? cur : (int64_t)ub;     // first byte not consumed by a complete record
-        // ---- shard limit: drop records starting at/after u_limit (host trims counts; offsets are sorted)
-        std::vector<uint32_t> rbase(nb + 1); uint64_t R = 0;
-        bool limited = u_limit < (int64_t)ub && !fix;        // (-m keeps the records behind the limit: they are marked as the next rank's by k2_decode)
-        std::vector<uint16_t> tmp_slots;
-        for (size_t i = 0; i < nb; i++) {
-            if (limited && cnt[i]) {
-                if (cstart[i] >= u_limit) cnt[i] = 0;
-                else if (cstart[i + 1] > u_limit) {   // partial: count slots below the limit
-                    tmp_slots.resize(cnt[i]);
-                    CK(cudaMemcpy(tmp_slots.data(), (uint16_t*)h->slots.p + sbase[i], cnt[i] * 2, cudaMemcpyDeviceToHost));
-                    uint32_t k = 0; while (k < cnt[i] && ((k == 0 || cstart[i] > 0) ? cstart[i] : 0) + tmp_slots[k] < u_limit) k++;     // slot encoding: see k2_walk
-                    cnt[i] = k;
-                }
-            }
-            rbase[i] = (uint32_t)R; R += cnt[i];
-        }
-        rbase[nb] = (uint32_t)R;
-        if (R > 0xFFFFFFF0ull) return fail(h, BDEPTH_ERR_ARG, "batch too large");
-        UP(h->count.p, cnt, nb * 4);
-        if (limited && last_batch && tail < u_limit && tail < (int64_t)ub && b1 < B.size()) return fail(h, BDEPTH_ERR_FORMAT, "record at the shard boundary spans more than %u BGZF blocks", SHARD_EXTRA_BLOCKS);
-        UP(h->rec_base.p, rbase.data(), (nb + 1) * 4);
-        st.n_records += R;
-        // ---- K2 decode
-        size_t Rc = R ? R : 1;
-        CK(h->soa_start.ensure(Rc * 8)); CK(h->soa_span.ensure(Rc * 4)); CK(h->soa_meta.ensure(Rc * 4)); CK(h->soa_off.ensure(Rc * 8)); CK(h->soa_ncl.ensure(Rc * 4)); CK(h->soa_lseq.ensure(Rc * 4)); CK(h->long_list.ensure(Rc * 4));
-        RecordSoA soa{h->soa_start.as<uint64_t>(), h->soa_span.as<uint32_t>(), h->soa_meta.as<uint32_t>(), h->soa_off.as<int64_t>(), h->soa_ncl.as<uint32_t>(), h->soa_lseq.as<int32_t>()};
-        ScanStats zs{0, 0, 0, 0, ~0ull, 0, 0, ~0ull, 0, 0, ~0ull, 0, ~0ull, ~0ull, 0};
-        const int64_t ghost_below = (fix && batch_no > 0) ? (int64_t)ghost_below_abs - (int64_t)batch_u0 : INT64_MIN;
-        const int64_t own_lo = (fix && h->world > 1) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;           // -m on several ranks: records outside belong to the neighbours
-        const int64_t own_hi = (fix && h->world > 1 && h->limit_abs_u < h->total_u) ? (int64_t)h->limit_abs_u - (int64_t)batch_u0 : INT64_MAX;
-        const int64_t zone_below = (!fix && !sparse && h->world > 1) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;       // records of the previous ranks' zone
-        UP(h->scan_stats.p, &zs, sizeof zs);
-        if ((mode == RUN_SCAN_ONLY || mode == RUN_INDEX || mode == RUN_FLAGSTAT || view) && !h->ref_has.p) { CK(h->ref_has.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has.p, 0, (nref / 32 + 2) * 4, sm)); }
-        // runs with -L regions: K2's every-passing-read bits go to a scratch word array, k_ref_seen marks the references of the reads that overlap a region
-        uint32_t* has_dst = h->ref_has.as<uint32_t>();
-        const uint32_t n_flt_k2 = mode == RUN_FULL ? (uint32_t)h->regions.size() : 0u;
-        if (n_flt_k2) {
-            if (!flt_uploaded) {
-                std::vector<uint64_t> fl; fl.reserve(2 * (size_t)n_flt_k2);
-                for (auto& g : h->regions) fl.push_back(h->hdr.ref_lin0[g.ref_id] + g.start);
-                for (auto& g : h->regions) fl.push_back(h->hdr.ref_lin0[g.ref_id] + g.end);
-                CK(h->flt_d.ensure(fl.size() * 8)); CK(cudaMemcpyAsync(h->flt_d.p, fl.data(), fl.size() * 8, cudaMemcpyHostToDevice, sm)); CK(cudaStreamSynchronize(sm));      // (fl is a local)
-                CK(h->ref_has_all.ensure((nref / 32 + 2) * 4)); CK(cudaMemsetAsync(h->ref_has_all.p, 0, (nref / 32 + 2) * 4, sm));
-                flt_uploaded = true;
-            }
-            has_dst = h->ref_has_all.as<uint32_t>();
-        }
-#define K2_DECODE(F, G) BD_LAUNCH((unsigned)((nb * 32 + 255) / 256), 256, 0, sm, k2_decode<F, G>)(sp, h->chunk_start.as<int64_t>(), (uint32_t)nb, h->slot_base.as<uint32_t>(), h->slots.as<uint16_t>(), h->count.as<uint32_t>(), h->rec_base.as<uint32_t>(), soa, h->mapq_gt, h->flag_reject, h->scan_stats.as<ScanStats>(), h->long_list.as<uint32_t>(), has_dst, rgt, d_fprog, ghost_below, own_lo, own_hi, zone_below)
-        if (fix) { if (d_fprog) K2_DECODE(true, true); else K2_DECODE(false, true); }
-        else if (d_fprog) K2_DECODE(true, false);
-        else K2_DECODE(false, false);
-#undef K2_DECODE
-        CK(cudaGetLastError()); st.gpu_launches++;
-        if (R && mode != RUN_INDEX && mode != RUN_SCAN_ONLY && mode != RUN_FLAGSTAT && !view) {      // quirk 1: CIGARs that begin with N, rewritten to what the reference's cursor makes of them (the index, the raw scan, flagstat and view see the file as it is)
-            // region mode proper (no window slots, no -m, one rank): the statistics of such a read are reproduced (kernels.cuh); otherwise refused
-            const bool lead_n_regions = h->seg.on && h->seg.n && !h->seg.has_u && !h->seg.has_min && !fix && h->world == 1;
-            LeadNSegs lsg{nullptr, nullptr, nullptr, nullptr, 0u, nullptr, nullptr, 1u, h->minq};
-            if (lead_n_regions) lsg = LeadNSegs{h->seg.s.as<uint64_t>(), h->seg.e.as<uint64_t>(), h->seg.pmax.as<uint64_t>(), h->seg.id.as<uint32_t>(), h->seg.n, h->seg.reads.as<uint32_t>(), h->seg.mbases.as<uint32_t>(),
-                                                (uint32_t)((h->combined || h->hdr.sample_names.size() <= 1) ? 1 : h->hdr.sample_names.size()), h->minq};
-            CK(h->lead_list.ensure(Rc * 4));
-            BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k2_lead_n_find)(soa, u0, (uint32_t)R, h->lead_list.as<uint32_t>(), h->scan_stats.as<ScanStats>());
-            BD_LAUNCH(32, 128, 0, sm, k2_lead_n_fix)(soa, u0, h->lead_list.as<uint32_t>(), h->scan_stats.as<ScanStats>(), (h->seg.on && !lead_n_regions) ? 1 : 0,
-                                                    n_flt_k2 ? h->flt_d.as<uint64_t>() : nullptr, n_flt_k2 ? h->flt_d.as<uint64_t>() + n_flt_k2 : nullptr, n_flt_k2, lsg);
-            CK(cudaGetLastError()); st.gpu_launches += 2;
-        }
-        if (n_flt_k2 && R) {
-            BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_ref_seen)(soa, (uint32_t)R, h->flt_d.as<uint64_t>(), h->flt_d.as<uint64_t>() + n_flt_k2, n_flt_k2, h->ref_lin0_d.as<uint64_t>(), (uint32_t)nref, h->ref_has.as<uint32_t>());
-            CK(cudaGetLastError()); st.gpu_launches++;
-        }
-        DOWN(ssp, ScanStats, h->scan_stats.p, sizeof(ScanStats));
-        CK(cudaEventRecord(e3, sm));
-        CK(cudaStreamSynchronize(sm));
-        const ScanStats ss = *ssp;
-        st.n_records -= ss.n_ghost + ss.n_ghost_right;          // re-read records of the previous batch / of the neighbours' zones are counted there
-        if (ss.bad_rec != ~0ull) return fail(h, BDEPTH_ERR_FORMAT, "corrupt BAM record (#%llu of the batch): its name, CIGAR, sequence and qualities do not fit its block_size", ss.bad_rec);
-        if (ss.lead_n != ~0ull) return fail(h, BDEPTH_ERR_FORMAT, "read #%llu of the batch: its CIGAR begins with N%s (pileup.d:180-189): there is no result to reproduce", ss.lead_n,
-                                             h->seg.on ? " -- the reference computes region / window statistics of such a read partly from its CIGAR as written and partly from a cursor that skips the leading N" : " and ends in a match -- the reference's pileup cursor runs past the read's sequence on such a read");
-        if (ss.rg_err != ~0ull) return fail(h, BDEPTH_ERR_FORMAT, "error in read #%llu of the batch: its read group is not present in the header", ss.rg_err);
-        st.n_records_pass += ss.n_pass; st.n_cigar_ops += ss.n_cigar; st.seq_bytes += ss.seq_bytes; st.long_reads += ss.n_long;
-        if (ss.n_pass) { shard_min = std::min<uint64_t>(shard_min, ss.min_start); shard_max = std::max<uint64_t>(shard_max, ss.max_end); }
-        if (mode == RUN_SCAN_ONLY) {
-            if (ro && R) {
-                uint64_t n = std::min<uint64_t>(R, ro->scan_cap > ro->scan_n ? ro->scan_cap - ro->scan_n : 0);
-                std::vector<uint64_t> hs(n), ho(n); std::vector<uint32_t> hsp(n), hm(n), hn(n);
-                CK(cudaMemcpy(hs.data(), soa.start, n * 8, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(ho.data(), soa.off, n * 8, cudaMemcpyDeviceToHost));
-                CK(cudaMemcpy(hsp.data(), soa.span, n * 4, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(hm.data(), soa.meta, n * 4, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(hn.data(), soa.ncl, n * 4, cudaMemcpyDeviceToHost));
-                for (uint64_t i = 0; i < n; i++) {
-                    uint64_t k = ro->scan_n + i; int32_t rid = -1, p = -1;
-                    if (hs[i] != START_UNPLACED) { size_t lo = 0, hi = nref; while (lo + 1 < hi) { size_t m = (lo + hi) / 2; if (h->hdr.ref_lin0[m] <= hs[i]) lo = m; else hi = m; } while (lo + 1 < nref && h->hdr.ref_lin0[lo + 1] <= hs[i] && h->hdr.ref_len[lo] == 0) lo++; rid = (int32_t)lo; p = (int32_t)(hs[i] - h->hdr.ref_lin0[lo]); }
-                    if (ro->ref_id) ro->ref_id[k] = rid; if (ro->pos) ro->pos[k] = p; if (ro->span) ro->span[k] = hsp[i];
-                    if (ro->flag) ro->flag[k] = (uint16_t)(hm[i] >> 16); if (ro->mapq) ro->mapq[k] = (uint8_t)(hm[i] >> 8); if (ro->n_cigar) ro->n_cigar[k] = (uint16_t)(hn[i] >> 8);
-                    if (ro->rec_off) ro->rec_off[k] = batch_u0 + ho[i] - 4;       // absolute offset of the block_size field
-                }
-            }
-            if (ro) ro->scan_n += R;
-        }
-        // ---- BAI builder: the per-record part of IndexBuilder.put (bai/indexing.d:290-333) for this sub-batch's records
-        if (mode == RUN_INDEX && R) {
-            auto& X = h->ix;
-            CK(X.runs.ensure(R * sizeof(IndexRun))); CK(X.excs.ensure(R * sizeof(IndexExc)));
-            BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_index_scan)(soa, u0, (uint32_t)R, (unsigned long long)batch_u0, (int)nref, X.lin_base.as<uint32_t>(), X.lin_cap.as<uint32_t>(), X.lin.as<unsigned long long>(), X.lin_len.as<uint32_t>(),
-                                                                               X.n_mapped.as<unsigned long long>(), X.n_unmapped.as<unsigned long long>(), X.carry.as<IndexCarry>(), X.runs.as<IndexRun>(), X.excs.as<IndexExc>(), X.ctl.as<IndexCtl>());
-            BD_LAUNCH(1, 32, 0, sm, k_index_carry)(soa, u0, (unsigned long long)batch_u0, X.carry.as<IndexCarry>(), X.ctl.as<IndexCtl>());
-            CK(cudaGetLastError()); st.gpu_launches += 2;
-            DOWN(icp, IndexCtl, X.ctl.p, sizeof(IndexCtl));
-            CK(cudaStreamSynchronize(sm));
-            const IndexCtl ic = *icp;
-            if (ic.bad_ref != ~0ull) return fail(h, BDEPTH_ERR_FORMAT, "record #%llu of the batch names a reference the header does not have", ic.bad_ref);
-            if (ic.unsorted != ~0ull) return fail(h, BDEPTH_ERR_FORMAT, "BAM file is not coordinate-sorted (record #%llu of the batch lies before the read in front of it)", ic.unsorted);
-            if (ic.past_end) return fail(h, BDEPTH_ERR_FORMAT, "%llu reads reach more than 16 kbp past the end of their reference: no index is built for such a file", ic.past_end);
-            if (ic.n_runs) { size_t o = X.h_runs.size(); X.h_runs.resize(o + ic.n_runs); CK(cudaMemcpy(X.h_runs.data() + o, X.runs.p, ic.n_runs * sizeof(IndexRun), cudaMemcpyDeviceToHost)); std::sort(X.h_runs.begin() + o, X.h_runs.end(), [](const IndexRun& a, const IndexRun& b) { return a.start_abs < b.start_abs; }); }
-            if (ic.n_exc) { size_t o = X.h_excs.size(); X.h_excs.resize(o + ic.n_exc); CK(cudaMemcpy(X.h_excs.data() + o, X.excs.p, ic.n_exc * sizeof(IndexExc), cudaMemcpyDeviceToHost)); std::sort(X.h_excs.begin() + o, X.h_excs.end(), [](const IndexExc& a, const IndexExc& b) { return a.start_abs < b.start_abs; }); }
-            CK(cudaMemsetAsync(X.ctl.p, 0, 16, sm));      // n_runs, n_exc
-        }
-        // ---- per-read segment counting (countRead, depth.d:661-669) for the window / region front ends
-        if (mode == RUN_FULL && h->seg.on && h->seg.n && ss.n_pass) {
-            if (h->minq) BD_LAUNCH((unsigned)((R + 127) / 128), 128, 0, sm, k_read_segments<true>)(soa, u0, (uint32_t)R, h->seg.s.as<uint64_t>(), h->seg.e.as<uint64_t>(), h->seg.pmax.as<uint64_t>(), h->seg.id.as<uint32_t>(), h->seg.has_min ? h->seg.minstart.as<uint64_t>() : nullptr, h->seg.n, h->seg.reads.as<uint32_t>(), h->minq, h->S, h->seg.has_min ? h->seg.bases_reads.as<uint32_t>() : nullptr);
-            else BD_LAUNCH((unsigned)((R + 127) / 128), 128, 0, sm, k_read_segments<false>)(soa, u0, (uint32_t)R, h->seg.s.as<uint64_t>(), h->seg.e.as<uint64_t>(), h->seg.pmax.as<uint64_t>(), h->seg.id.as<uint32_t>(), h->seg.has_min ? h->seg.minstart.as<uint64_t>() : nullptr, h->seg.n, h->seg.reads.as<uint32_t>(), 0, h->S, h->seg.has_min ? h->seg.bases_reads.as<uint32_t>() : nullptr);
-            CK(cudaGetLastError()); st.gpu_launches++;
-        }
-        uint64_t idx_tiles_base = 0; uint32_t idx_n_tiles = 0;      // K3's per-tile read index of this sub-batch (the mate kernels look reads up through it)
-        // ---- K3
-        uint64_t gmin = std::min<uint64_t>(ss.min_start, ss.min_start_all), gmax = ss.max_end;
-        if (ss.n_zone_pass && gmin < h->cnt_base) gmin = h->cnt_base;      // a zone read may begin before the window; only what reaches this rank's positions matters
-        // (a sub-batch of the zone's first blocks can hold nothing but reads that end before this rank's first position -- the linear index
-        // points at the first read that overlaps the 16 kbp window, the short reads behind it need not: nothing to count then)
-        if (mode == RUN_FULL && (ss.n_pass || ss.n_zone_pass) && gmax > gmin) {
-            if (gmin < h->cnt_base || gmax > h->cnt_base + h->win_len) {
-                // the index does not describe this file (the reference only checks that one exists, depth.d:1166):
-                // start over with the whole genome as the counter window
-                if (!h->bai_window_ok) return fail(h, BDEPTH_ERR_FORMAT, "read extends past the end of the reference space");
-                h->bai_window_ok = false; CK(cudaDeviceSynchronize());
-                if (h->force_window || h->accum) return RC_RETRY_WINDOW;      // several inputs: the caller starts over with the whole genome as the window
-                return run_pipeline(h, mode, ro, em);
-            }
-            uint64_t t_lo = (gmin - h->cnt_base) / TILE_POS, t_hi = (gmax - h->cnt_base + TILE_POS - 1) / TILE_POS;
-            uint64_t n_tiles = t_hi - t_lo; uint64_t tiles_base = h->cnt_base + t_lo * TILE_POS;
-            idx_tiles_base = tiles_base; idx_n_tiles = (uint32_t)n_tiles;
-            if (t_hi * TILE_POS > h->win_len) return fail(h, BDEPTH_ERR_FORMAT, "read extends past the end of the reference space");
-            CK(h->tile_first.ensure((n_tiles + 2) * 4)); CK(h->tile_lo.ensure((n_tiles + 2) * 4));
-            BD_LAUNCH((unsigned)((n_tiles + 2 + 255) / 256), 256, 0, sm, k_fill_u32)(h->tile_first.as<uint32_t>(), (uint32_t)R, n_tiles + 2);
-            CK(cudaMemsetAsync(h->tile_lo.p, 0xFF, (n_tiles + 2) * 4, sm));
-            if (h->want_presence) { BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_presence)(soa, (uint32_t)R, h->cnt_base, h->win_len, h->present.as<uint32_t>()); st.gpu_launches++; }
-            BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k3_tile_index)(soa, (uint32_t)R, tiles_base, (uint32_t)n_tiles, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>());
-            CK(cudaGetLastError()); st.gpu_launches += 2;
-            for (uint32_t si = 0; si < h->S; si++) {      // one counter set per sample (one pass when combined / single sample)
-                uint32_t* cnt = h->counts.as<uint32_t>() + (uint64_t)si * N_PLANES * h->win_len; int sel = h->S > 1 ? (int)si : -1;
-                if (ss.n_long) {
-                    if (h->minq) BD_LAUNCH((unsigned)((ss.n_long * 32 + 255) / 256), 256, 0, sm, k3_scatter_long<true>)(soa, u0, h->long_list.as<uint32_t>(), (uint32_t)ss.n_long, h->cnt_base, h->win_len, cnt, h->minq, sel);
-                    else BD_LAUNCH((unsigned)((ss.n_long * 32 + 255) / 256), 256, 0, sm, k3_scatter_long<false>)(soa, u0, h->long_list.as<uint32_t>(), (uint32_t)ss.n_long, h->cnt_base, h->win_len, cnt, 0, sel);
-                    CK(cudaGetLastError()); st.gpu_launches++;
-                }
-                if (h->k3_tile) {      // CTA per tile, shared-memory counters, records staged by cp.async.bulk
-                    if (h->minq) BD_LAUNCH((unsigned)n_tiles, 256, K3T_SMEM, sm, k3_tile<true>)(soa, u0, (int64_t)ub, (uint32_t)R, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, h->minq, sel);
-                    else BD_LAUNCH((unsigned)n_tiles, 256, K3T_SMEM, sm, k3_tile<false>)(soa, u0, (int64_t)ub, (uint32_t)R, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, 0, sel);
-                } else if (h->k3_pre) {       // round-1 gather kernel with lane-parallel record prefetch (BDEPTH_K3=gather)
-                    if (h->minq) BD_LAUNCH((unsigned)n_tiles, 256, 0, sm, k3_gather<true, true>)(soa, u0, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, h->minq, sel);
-                    else BD_LAUNCH((unsigned)n_tiles, 256, 0, sm, k3_gather<false, true>)(soa, u0, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, 0, sel);
-                } else if (h->minq) BD_LAUNCH((unsigned)n_tiles, 256, 0, sm, k3_gather<true, false>)(soa, u0, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, h->minq, sel);
-                else BD_LAUNCH((unsigned)n_tiles, 256, 0, sm, k3_gather<false, false>)(soa, u0, tiles_base, h->cnt_base, h->win_len, h->tile_first.as<uint32_t>(), h->tile_lo.as<uint32_t>(), cnt, 0, sel);
-                CK(cudaGetLastError()); st.gpu_launches++;
-            }
-        }
-        // ---- -m: take the worse mate of every overlapping pair out again (mates.cuh)
-        if (fix) {      // where the next batch's stream begins if nothing is open: the first record this batch did not consume
-            const uint64_t tail_abs = batch_u0 + (uint64_t)tail; size_t lo = 0, hi = B.size(); while (lo + 1 < hi) { size_t m2 = (lo + hi) / 2; if (B[m2].uoff <= tail_abs) lo = m2; else hi = m2; }
-            ghost_b = lo; ghost_entry = (int64_t)(tail_abs - B[lo].uoff); ghost_below_abs = tail_abs;
-        }
-        if (fix && R && (ss.n_pass || ss.n_ghost || ss.n_ghost_right)) {
-            if (subs.size() != 1) return fail(h, BDEPTH_ERR_ARG, "internal: fix-mate-overlaps scans a batch as a whole");
-            uint64_t s_last = 0;       // start of the batch's last record: nothing that follows starts before it
-            CK(cudaMemcpyAsync(&s_last, soa.start + (R - 1), 8, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
-            cudaEvent_t em0 = h->ev[20], em1 = h->ev[21];
-            CK(cudaEventRecord(em0, sm));
-            CK(h->m_hash.ensure(Rc * 8)); CK(h->m_flag.ensure(Rc * 4)); CK(h->m_ctl.ensure(64));
-            std::vector<uint64_t> fl;                 // -L: merged regions (sorted, disjoint) in linear coordinates, starts then ends
-            for (auto& g : h->regions) fl.push_back(h->hdr.ref_lin0[g.ref_id] + g.start);
-            for (auto& g : h->regions) fl.push_back(h->hdr.ref_lin0[g.ref_id] + g.end);
-            const uint32_t n_flt = (uint32_t)h->regions.size();
-            CK(h->m_flt.ensure(fl.size() * 8 + 16));
-            if (n_flt) CK(cudaMemcpyAsync(h->m_flt.p, fl.data(), fl.size() * 8, cudaMemcpyHostToDevice, sm));
-            CK(cudaMemsetAsync(h->m_ctl.p, 0, 64, sm)); CK(cudaMemsetAsync((uint8_t*)h->m_ctl.p + 48, 0xFF, 16, sm));       // err, stat; open_off = open_start = none
-            const bool segm = h->seg.on && h->seg.n;
-            MateParams mp{soa.start, soa.span, soa.meta, soa.off, soa.ncl, soa.lseq, u0, (uint32_t)R, h->m_hash.as<uint64_t>(), h->m_flag.as<uint32_t>(),
-                          h->m_flt.as<uint64_t>(), h->m_flt.as<uint64_t>() + n_flt, n_flt, h->counts.as<uint32_t>(), h->cnt_base, h->win_len, h->S, h->minq,
-                          segm ? h->seg.s.as<uint64_t>() : nullptr, segm ? h->seg.e.as<uint64_t>() : nullptr, segm ? h->seg.pmax.as<uint64_t>() : nullptr, segm ? h->seg.id.as<uint32_t>() : nullptr,
-                          segm ? h->seg.n : 0u, segm ? h->seg.reads.as<uint32_t>() : nullptr, segm ? h->seg.mbases.as<uint32_t>() : nullptr, h->S,
-                          segm && h->seg.has_u ? h->seg.ustart.as<uint64_t>() : nullptr, segm && h->seg.has_u && h->seg.has_min ? h->seg.minstart.as<uint64_t>() : nullptr, segm && h->seg.has_u ? h->seg.ext_max : 0ull,
-                          h->tile_lo.as<uint32_t>(), idx_tiles_base, idx_n_tiles, h->long_list.as<uint32_t>(), (uint32_t)ss.n_long,
-                          (uint32_t)ss.n_ghost, s_last, prev_s_last, covered_from, last_batch ? 1 : 0, (unsigned long long*)((uint8_t*)h->m_ctl.p + 48), (unsigned long long*)((uint8_t*)h->m_ctl.p + 56),
-                          (last_batch && blk_hi < B.size()) ? 1 : 0, (unsigned long long*)((uint8_t*)h->m_ctl.p + 40), (uint32_t)ss.n_ghost_right, ghost_below == INT64_MIN ? INT64_MIN : ghost_below + 4, 0,
-                          (int*)h->m_ctl.p, (unsigned long long*)((uint8_t*)h->m_ctl.p + 16)};
-            const unsigned mg = (unsigned)((R + 127) / 128);
-            BD_LAUNCH(mg, 128, 0, sm, km_hash)(mp); BD_LAUNCH(mg, 128, 0, sm, km_link)(mp); BD_LAUNCH(mg, 128, 0, sm, km_fix)(mp);
-            if (!last_batch) { BD_LAUNCH(mg, 128, 0, sm, km_cover)(mp); st.gpu_launches++; }
-            CK(cudaGetLastError()); st.gpu_launches += 3;
-            CK(cudaEventRecord(em1, sm));
-            struct { int err[4]; unsigned long long stat[3]; unsigned long long fix_max_end; unsigned long long open_off, open_start; } ctl;
-            CK(cudaMemcpyAsync(&ctl, h->m_ctl.p, sizeof ctl, cudaMemcpyDeviceToHost, sm));
-            CK(cudaStreamSynchronize(sm));
-            if (ctl.err[0] == MATE_ERR_TOO_MANY) return fail(h, BDEPTH_ERR_ARG, "fix-mate-overlaps: more than %d reads of one name cover one position (record #%d of the batch)", MATE_MAX_MEMBERS, ctl.err[1]);
-            if (ctl.err[0] == MATE_ERR_CROSS) return fail(h, BDEPTH_ERR_ARG, "fix-mate-overlaps: four or more overlapping reads of one name next to a batch boundary (record #%d of the batch): not reproduced there, use larger batches", ctl.err[1]);
-            st.mate_pairs += ctl.stat[0]; st.mate_pair_columns += ctl.stat[1]; st.mate_groups += ctl.stat[2];
-            if (!last_batch && ctl.open_off != ~0ull && batch_u0 + (ctl.open_off - 4) < ghost_below_abs) {      // something is still open: re-read from its first record
-                const uint64_t g_abs = batch_u0 + (ctl.open_off - 4); size_t lo = 0, hi = B.size(); while (lo + 1 < hi) { size_t m2 = (lo + hi) / 2; if (B[m2].uoff <= g_abs) lo = m2; else hi = m2; }
-                ghost_b = lo; ghost_entry = (int64_t)(g_abs - B[lo].uoff);
-            }
-            if (ctl.err[0] == MATE_ERR_ZONE) return fail(h, BDEPTH_ERR_ARG, "fix-mate-overlaps on several ranks: overlapping reads of one name reach more than %u BGZF blocks past a shard boundary (record #%d of the batch)", MATE_ZONE_BLOCKS, ctl.err[1]);
-            if (ctl.fix_max_end > shard_max && shard_min != UINT64_MAX) shard_max = ctl.fix_max_end;      // the halo exchange carries the corrections to their owners
-            prev_s_last = s_last; covered_from = ctl.open_start;
-            { float t = 0; CK(cudaEventElapsedTime(&t, em0, em1)); st.ms_mates += t; }
-        }
-        CK(cudaEventRecord(e4, sm));
-        // ---- flagstat: the sub-batch's records into the 26 counters (records of the previous rank's zone are that rank's)
-        if (mode == RUN_FLAGSTAT && R) {
-            const int64_t own_from = h->world > 1 ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;
-            CK(cudaEventRecord(h->ev[22], sm));
-            BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_flagstat)(soa, u0, (uint32_t)R, own_from, h->fs.as<unsigned long long>());
-            CK(cudaGetLastError()); st.gpu_launches++;
-            CK(cudaEventRecord(h->ev[23], sm));
-        }
-        // ---- view -c: the sub-batch's selected records into the count (a sparse run on several ranks has no zone: each rank reads its own chunks)
-        if (mode == RUN_VIEW_COUNT && R) {
-            const int64_t own_from = (h->world > 1 && !sparse) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;
-            CK(cudaEventRecord(h->ev[22], sm));
-            BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_view_count)(soa, u0, (uint32_t)R, own_from, h->vsel, h->vc.as<unsigned long long>());
-            CK(cudaGetLastError()); st.gpu_launches++;
-            CK(cudaEventRecord(h->ev[23], sm));
-        }
-        // ---- view: the SAM lines of the sub-batch's selected records, handed out before the inflate buffer is reused
-        if (mode == RUN_VIEW_TEXT && R) {
-            const int64_t own_from = (h->world > 1 && !sparse) ? (int64_t)h->own_lo_abs_u - (int64_t)batch_u0 : INT64_MIN;
-            rc = view_text_sub(h, soa, u0, (uint32_t)R, own_from); if (rc) return rc;
-        }
-        // Progressive delivery: positions below the start of the sub-batch's last own read are final (the file is coordinate sorted).  Several ranks
-        // (plain shards): a rank's own positions begin at its first passing read -- known once such a read has been seen -- and the reads of the
-        // previous ranks that reach into them come first in its stream (the zone), so the same holds; where its positions end it learns at the end.
-        const bool zone_mode = h->world > 1 && h->comm && !fix && !sparse;
-        if (em && zone_mode && h->rank > 0 && shard_min != UINT64_MAX) em->lo_clip = shard_min;
-        if (em && mode == RUN_FULL && (h->world == 1 || (zone_mode && (h->rank == 0 || shard_min != UINT64_MAX))) && !fix && !last_batch && ss.n_pass) { int rce = em->advance(ss.max_start / TILE_POS * TILE_POS, e4); if (rce) return rce; }
+        if (rc) return rc;
         // ---- carry the incomplete tail record to the front of the next batch
-        uint64_t new_carry = (uint64_t)((int64_t)ub - tail);
+        uint64_t new_carry = (uint64_t)((int64_t)s.ub - s.tail);
         // the file ends inside a record: readExact throws "not enough data in stream" (readrange.d:169); fewer than 4 left-over bytes end the stream quietly (:139-149)
-        if (last_batch && last_sub && !sparse && !limited && b1 == B.size() && new_carry >= 4) return fail(h, BDEPTH_ERR_FORMAT, "truncated BAM record at the end of the file (not enough data in stream)");
-        if (!last_batch && last_sub && new_carry && !fix) {      // inside a batch the tail already sits right below the next sub-batch; -m re-reads it with the next batch
+        if (s.last_batch && !sparse && !s.limited && sb1 == B.size() && new_carry >= 4) return fail(h, BDEPTH_ERR_FORMAT, "truncated BAM record at the end of the file (not enough data in stream)");
+        if (!s.last_batch && s.last_sub && new_carry && !fix) {      // inside a batch the tail already sits right below the next sub-batch; -m re-reads it with the next batch
             if (new_carry > CARRY_MAX) return fail(h, BDEPTH_ERR_FORMAT, "BAM record larger than %zu bytes", CARRY_MAX);
-            CK(cudaMemcpyAsync(m_u0 - new_carry, u0 + tail, new_carry, cudaMemcpyDeviceToDevice, sm));
+            CK(cudaMemcpyAsync(m_u0 - new_carry, s.u0 + s.tail, new_carry, cudaMemcpyDeviceToDevice, sm));
         }
         CK(cudaStreamSynchronize(sm));
-        if ((mode == RUN_FLAGSTAT || mode == RUN_VIEW_COUNT) && R) { float t; CK(cudaEventElapsedTime(&t, h->ev[22], h->ev[23])); ms_census += t; }
-        { float t; if (!h->staged && last_sub) { CK(cudaEventElapsedTime(&t, h->ev[18 + (batch_no & 1)], h->ev[14 + (batch_no & 1)])); ms_h2d += t; } if (last_sub) { CK(cudaEventElapsedTime(&t, e1, e2)); ms_k1 += t; } CK(cudaEventElapsedTime(&t, e2, e3)); ms_k2 += t; CK(cudaEventElapsedTime(&t, e3, e4)); ms_k3 += t; }
-        carry_len = (last_batch || fix) ? 0 : new_carry; first_batch = false;
+        if (P.census_timed) { float t; CK(cudaEventElapsedTime(&t, h->ev[22], h->ev[23])); P.ms_census += t; P.census_timed = false; }
+        { float t; if (!h->staged && s.last_sub) { CK(cudaEventElapsedTime(&t, h->ev[18 + (batch_no & 1)], h->ev[14 + (batch_no & 1)])); ms_h2d += t; } if (s.last_sub) { CK(cudaEventElapsedTime(&t, e1, e2)); ms_k1 += t; } CK(cudaEventElapsedTime(&t, e2, e3)); ms_k2 += t; CK(cudaEventElapsedTime(&t, e3, e4)); ms_k3 += t; }
+        P.carry_len = (s.last_batch || fix) ? 0 : new_carry; P.first_batch = false;
         hs.used = 0;      // synchronised above: the scratch is free again
         }   // sub-batches
         if (sparse_bad) break;
@@ -1368,40 +1435,29 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             uint32_t flag = sparse_bad ? 1u : 0u;
             CK(cudaMemcpyAsync(h->misc.p, &flag, 4, cudaMemcpyHostToDevice, sm));
             NK(nccl().AllReduce(h->misc.p, h->misc.p, 1, NCCL_UINT32, NCCL_SUM, h->comm, sm));
-            h->coll_pending = view ? 4 : 1;
+            h->coll_pending = need.owes;
             CK(cudaMemcpyAsync(&flag, h->misc.p, 4, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
-            if (flag >= SPARSE_PEER_FAILED) { h->coll_pending = 0; return fail(h, BDEPTH_ERR_NCCL, "another rank of the run stopped with an error (its own message says why): no result"); }
+            if (flag >= SPARSE_PEER_FAILED) { h->coll_pending = Owed::NOTHING; return fail(h, BDEPTH_ERR_NCCL, "%s", MSG_PEER_STOPPED); }
             sparse_bad = flag != 0;
-        } else if (sparse_bad) return fail(h, BDEPTH_ERR_FORMAT, "the index does not describe this file (a region chunk does not end at a record); several ranks without a NCCL id cannot fall back together");
-        if (sparse_bad && mode == RUN_VIEW_TEXT) { h->coll_pending = 4; return fail(h, BDEPTH_ERR_FORMAT, "the index does not describe this file (a region chunk does not end at a record), found after SAM lines were delivered"); }
-        if (sparse_bad) { h->sparse_ok = false; CK(cudaDeviceSynchronize()); return run_pipeline(h, mode, ro, em); }
+        } else if (sparse_bad) return fail(h, BDEPTH_ERR_FORMAT, "%s; several ranks without a NCCL id cannot fall back together", MSG_CHUNK_MISMATCH);
+        if (sparse_bad && mode == RUN_VIEW_TEXT) return refuse_index_after_text(h);      // (the view sum is still owed: abort_collectives joins it)
+        if (sparse_bad) { h->sparse_ok = false; CK(cudaDeviceSynchronize()); return RC_RESTART; }
     }
     st.ms_h2d = ms_h2d; st.ms_inflate = ms_k1; st.ms_scan = ms_k2; st.ms_coverage = ms_k3;
-    if (mode == RUN_FLAGSTAT) {      // several ranks: one all-reduce of the counters; a rank that failed has joined it with its "failed" word set (abort_collectives)
-        if (h->world > 1 && h->comm) { NK(nccl().AllReduce(h->fs.p, h->fs.p, FS_WORDS + 1, NCCL_UINT64, NCCL_SUM, h->comm, sm)); h->coll_pending = 0; }
-        CK(hs.ensure(16384)); hs.used = 0;      // (nothing is in flight: every sub-batch ended synchronised; a run without records has not sized it yet)
-        DOWN(fsp, uint64_t, h->fs.p, (FS_WORDS + 1) * 8);
-        CK(cudaStreamSynchronize(sm));
-        memcpy(h->fs_host, fsp, sizeof h->fs_host);
-        if (h->fs_host[FS_WORDS]) return fail(h, BDEPTH_ERR_NCCL, "another rank of the run stopped with an error (its own message says why): no result");
-        st.ms_reduce = ms_census;
-    }
-    if (mode == RUN_VIEW_TEXT) { rc = view_text_flush(h); if (rc) return rc; st.ms_d2h = h->vt.ms_d2h; }      // the last piece, before the ranks learn that this one is complete
-    if (view) {      // several ranks: one all-reduce of the count and the "failed" word (abort_collectives), as for flagstat
-        if (h->world > 1 && h->comm) { NK(nccl().AllReduce(h->vc.p, h->vc.p, 2, NCCL_UINT64, NCCL_SUM, h->comm, sm)); h->coll_pending = 0; }
-        CK(hs.ensure(16384)); hs.used = 0;
-        DOWN(vcp, uint64_t, h->vc.p, 16);
-        CK(cudaStreamSynchronize(sm));
-        memcpy(h->vc_host, vcp, sizeof h->vc_host);
-        if (h->vc_host[1]) return fail(h, BDEPTH_ERR_NCCL, "another rank of the run stopped with an error (its own message says why): no result");
-        st.ms_reduce = mode == RUN_VIEW_TEXT ? h->vt.ms_fmt : ms_census;
-    }
-    st.positions = mode == RUN_FULL ? h->hdr.total_len : 0;
     h->own_lo = 0; h->own_hi = h->hdr.total_len;
-    if (mode == RUN_FULL) {
-        if (h->world > 1 && h->comm) { rc = exchange_boundaries(h, shard_min, shard_max, sparse || fix); if (rc) return rc; }      // plain shards: the boundary table only (every rank counted its zone)
-        h->ref_has_host.assign(nref / 32 + 2, 0);
-        CK(cudaMemcpyAsync(h->ref_has_host.data(), h->ref_has.p, (nref / 32 + 2) * 4, cudaMemcpyDeviceToHost, sm));
+    switch (mode) {
+        case RUN_FLAGSTAT: case RUN_VIEW_COUNT: rc = finish_census(h, need.owes); if (rc) return rc; st.ms_reduce = P.ms_census; break;
+        case RUN_VIEW_TEXT:
+            rc = view_text_flush(h); if (rc) return rc;      // the last piece, before the ranks learn that this one is complete
+            st.ms_d2h = h->vt.ms_d2h; rc = finish_census(h, need.owes); if (rc) return rc; st.ms_reduce = h->vt.ms_fmt;
+            break;
+        case RUN_FULL:
+            st.positions = h->hdr.total_len;
+            if (h->world > 1 && h->comm) { rc = exchange_boundaries(h, P.shard_min, P.shard_max, sparse || fix); if (rc) return rc; }      // plain shards: the boundary table only (every rank counted its zone)
+            h->ref_has_host.assign(h->hdr.ref_len.size() / 32 + 2, 0);
+            CK(cudaMemcpyAsync(h->ref_has_host.data(), h->ref_has.p, (h->hdr.ref_len.size() / 32 + 2) * 4, cudaMemcpyDeviceToHost, sm));
+            break;
+        default: break;
     }
     CK(cudaEventRecord(h->ev[11], sm));
     CK(cudaStreamSynchronize(sm));
@@ -1409,6 +1465,12 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     st.own_lo = h->own_lo; st.own_hi = h->own_hi;
     st.host_wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count();
     return 0;
+}
+
+int run_pipeline(bdepth* h, RunMode mode, RunOut* ro, Emitter* em = nullptr) {
+    int rc; do rc = run_pipeline_body(h, mode, ro, em); while (rc == RC_RESTART);      // (a restart begins with nothing owed: the new run sets that up)
+    if (rc && rc != RC_RETRY_WINDOW) abort_collectives(h);
+    return rc;
 }
 
 // ---- several inputs --------------------------------------------------------------------------------------------------------
@@ -1578,7 +1640,7 @@ void bdepth_close(bdepth_t* h) {
     h->text[0].release(); h->text[1].release(); h->text_tiles.release(); h->text_offs.release(); h->text_zero.release(); h->text_samp.release(); h->present.release();
     h->seg.s.release(); h->seg.e.release(); h->seg.pmax.release(); h->seg.id.release(); h->seg.reads.release(); h->seg.minstart.release(); h->seg.bases_reads.release(); h->seg.mbases.release(); h->seg.ustart.release(); h->seg.dscr.release(); h->seg.da.release(); h->seg.dac.release(); h->seg.db.release(); h->seg.dthr.release(); h->seg.dbases.release(); h->seg.dcov.release();
     { auto& X = h->ix; X.lin.release(); X.lin_len.release(); X.lin_base.release(); X.lin_cap.release(); X.n_mapped.release(); X.n_unmapped.release(); X.carry.release(); X.ctl.release(); X.runs.release(); X.excs.release(); }
-    h->m_hash.release(); h->m_flag.release(); h->m_flt.release(); h->m_ctl.release(); h->fprog_d.release();
+    h->m_hash.release(); h->m_flag.release(); h->m_ctl.release(); h->fprog_d.release();
     h->vc.release(); h->vc_reg.release(); h->vc_prog.release();
     { auto& V = h->vt; V.names.release(); V.len.release(); V.off.release(); V.tiles.release(); V.ctl.release(); V.cut_r.release(); V.cut_o.release(); V.slot[0].release(); V.slot[1].release(); if (V.host) cudaFreeHost(V.host); V.host = nullptr; V.cap = 0; }
     if (h->comm) { nccl().CommDestroy(h->comm); h->comm = nullptr; }
@@ -1700,14 +1762,21 @@ static inline void owned_window(const bdepth* h, uint64_t& a, uint64_t& b) {
     const uint64_t lo = std::max(h->own_lo, h->cnt_base), hi = std::min(h->own_hi, h->cnt_base + h->win_len);
     if (hi > lo) { a = lo - h->cnt_base; b = hi - h->cnt_base; } else { a = b = 0; }
 }
-
-int bdepth_run_resident(bdepth_t* h) {
-    int rc = run_all_inputs(h); if (rc) return rc;
+// The covered positions (rows of default `depth base`) of the range this rank owns: k_count_covered and the copy of its sum are queued on
+// the main stream; *cov holds the count after the stream's next synchronisation.
+static int count_covered(bdepth* h, unsigned long long* cov) {
     cudaStream_t sm = h->s_main;
     CK(cudaMemsetAsync(h->misc.p, 0, 8, sm));
     uint64_t a, b; owned_window(h, a, b);
     if (b > a) { BD_LAUNCH(COUNT_GRID, 256, 0, sm, k_count_covered)(h->counts.as<uint32_t>(), h->win_len, a, b, (unsigned long long*)h->misc.p, N_PLANES * (int)h->S); CK(cudaGetLastError()); h->st.gpu_launches++; }
-    unsigned long long cov = 0; CK(cudaMemcpyAsync(&cov, h->misc.p, 8, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
+    CK(cudaMemcpyAsync(cov, h->misc.p, 8, cudaMemcpyDeviceToHost, sm));
+    return 0;
+}
+
+int bdepth_run_resident(bdepth_t* h) {
+    int rc = run_all_inputs(h); if (rc) return rc;
+    unsigned long long cov = 0; rc = count_covered(h, &cov); if (rc) return rc;
+    CK(cudaStreamSynchronize(h->s_main));
     h->st.covered_positions = cov;
     h->st.ms_total_device = h->st.ms_h2d + h->st.ms_inflate + h->st.ms_scan + h->st.ms_coverage + h->st.ms_exchange;
     return 0;
@@ -1724,11 +1793,7 @@ int bdepth_run_base(bdepth_t* h, bdepth_tile_cb cb, void* user) {
     rc = run_all_inputs(h, &em); if (rc) { em.finish(); return rc; }
     cudaStream_t sm = h->s_main;
     cudaEvent_t e0 = h->ev[5], e1 = h->ev[6];
-    // covered positions (rows of default `depth base`), over the range this rank owns
-    CK(cudaMemsetAsync(h->misc.p, 0, 8, sm));
-    { uint64_t ca, cb2; owned_window(h, ca, cb2);
-      if (cb2 > ca) { BD_LAUNCH(COUNT_GRID, 256, 0, sm, k_count_covered)(h->counts.as<uint32_t>(), h->win_len, ca, cb2, (unsigned long long*)h->misc.p, N_PLANES * (int)h->S); CK(cudaGetLastError()); h->st.gpu_launches++; } }
-    unsigned long long cov = 0; CK(cudaMemcpyAsync(&cov, h->misc.p, 8, cudaMemcpyDeviceToHost, sm));
+    unsigned long long cov = 0; rc = count_covered(h, &cov); if (rc) return rc;
     CK(cudaEventRecord(e0, sm));
     if (h->world > 1) { em.lo_clip = h->own_lo; em.hi_clip = h->own_hi; }      // multi-GPU: ranks deliver disjoint, ordered pieces (what was delivered on the way lies inside)
     rc = em.advance(UINT64_MAX, e0); if (rc) { em.finish(); return rc; }
@@ -1753,10 +1818,7 @@ int bdepth_run_base_text(bdepth_t* h, const bdepth_text_opts* o, bdepth_text_cb 
     cudaStream_t sm = h->s_main;
     cudaEvent_t e0 = h->ev[5], e1 = h->ev[6];
     CK(cudaEventRecord(e0, sm));
-    CK(cudaMemsetAsync(h->misc.p, 0, 8, sm));
-    { uint64_t ca, cb2; owned_window(h, ca, cb2);
-      if (cb2 > ca) { BD_LAUNCH(COUNT_GRID, 256, 0, sm, k_count_covered)(h->counts.as<uint32_t>(), h->win_len, ca, cb2, (unsigned long long*)h->misc.p, N_PLANES * (int)h->S); CK(cudaGetLastError()); h->st.gpu_launches++; } }
-    unsigned long long cov = 0; CK(cudaMemcpyAsync(&cov, h->misc.p, 8, cudaMemcpyDeviceToHost, sm));
+    unsigned long long cov = 0; rc = count_covered(h, &cov); if (rc) return rc;
     TextParams tp; memset(&tp, 0, sizeof tp);
     tp.min_cov = o->min_cov; tp.max_cov = o->max_cov; tp.annotate = o->annotate ? 1 : 0; tp.with_sample = h->combined ? 0 : 1;
     const std::string& sn = h->hdr.sample_names[0];
@@ -2121,11 +2183,7 @@ int bdepth_run_flagstat(bdepth_t* h, bdepth_flagstat* out) {
     return 0;
 }
 
-// ---- view -c ----------------------------------------------------------------------------------------------------------------------
-// ReadCounter over view_main's selection (sambamba/view.d:265-368): K1 + K2 as in every run, then k_view_count per sub-batch.  Regions on a
-// coordinate-sorted file with a usable index stage only their BAI chunks (plan_sparse, with the view's regions in place of the handle's for the
-// duration of the run); otherwise every record of the file is scanned.  The handle's depth settings are not used and stay as they were.
-// The selection of one view run into h->vsel and what to stage into `plan`: the flag bits, -s, -F from o, the regions regs[0, n_regs) read as
+// ---- view: the selection of one view run into h->vsel and what to stage into `plan`: the flag bits, -s, -F from o, the regions regs[0, n_regs) read as
 // o->regions_from says, and n_star '*' queries.  *empty: the run selects nothing (-L naming no region of a sorted file).
 int view_setup(bdepth* h, const bdepth_view_opts* o, const bdepth_region* regs, size_t n_regs, uint32_t n_star, std::vector<bdepth_region>& plan, bool* empty) {
     const bool positional = o->regions_from == BDEPTH_VIEW_POSITIONAL;

@@ -80,6 +80,23 @@ def test_foreign_index_falls_back_to_the_whole_file(big, tmp_path):
     assert np.array_equal(got, want)
 
 
+def test_foreign_index_restarts_before_the_last_batch(tmp_path):
+    # The index of the file's first ten reads bounds the counter window far too tightly: a read of the first sub-batch falls outside it and
+    # the run starts over with the whole genome as its window, while later batches and sub-batches of the first run are still ahead.
+    import sambamba_b200 as sb
+    reads = [(0, 20 * i, 30, 0, [(40, 0)], "ACGTA" * 8, "r%d" % i) for i in range(4000)]
+    p = helpers.write_bam(str(tmp_path / "f.bam"), [("r0", 90000)], reads, block=4096, bins="auto", index=False)
+    head = helpers.write_bam(str(tmp_path / "head.bam"), [("r0", 90000)], reads[:10], block=4096, bins="auto", index=False)
+    with sb.BDepth(head) as b:
+        open(p + ".bai", "wb").write(b.build_index())
+    want, _ = helpers.oracle_counts(p)
+    with sb.BDepth(p) as b:
+        b.set_tuning(1 << 16, 2)
+        got = b.run_base()
+        st = b.stats()
+    assert np.array_equal(got, want) and st["n_batches"] > 1 and st["n_records"] == 4000, st
+
+
 def test_lazy_open_frames_only_what_a_region_query_needs(big, tmp_path):
     """bdepth_open_lazy: a region query must not depend on BGZF members outside its BAI chunks.  A copy of the file whose
     LAST data member is damaged cannot be opened eagerly, but answers a query on its first reference when opened lazily --
