@@ -25,6 +25,8 @@
  *     (filters, -L, regions, '*')        utils/view/alignmentrangeprocessor.d:42-50
  *   SamSerializer over view_main's reads sambamba/view.d:265-379,        bdepth_run_view_text (`sambamba view`, SAM lines)
  *     (BamRead.toSam per read)           utils/view/alignmentrangeprocessor.d:97-106
+ *   JsonSerializer over view_main's     sambamba/view.d:265-379,        bdepth_run_view_json (`sambamba view -f json`)
+ *     reads (BamRead.toJson per read)    utils/view/alignmentrangeprocessor.d:149-158
  *
  * Conventions: every entry returns 0 on success or a negative bdepth_status; the message is
  * available through bdepth_last_error().  No exception crosses the boundary.  There is no CPU
@@ -299,6 +301,14 @@ int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* opts, uint64_t* c
  * the join is complete (BDEPTH_ERR_NCCL otherwise); positional regions there, and bdepth_add_input handles, are BDEPTH_ERR_ARG.
  * Timings: ms_inflate, ms_scan, ms_reduce (formatting kernels), ms_d2h (text copies), summed over the runs of a positional query. */
 int bdepth_run_view_text(bdepth_t* h, const bdepth_view_opts* opts, bdepth_text_cb cb, void* user);
+/* `sambamba view -f json` without -h or -H: exactly what JsonSerializer (utils/view/alignmentrangeprocessor.d:149-158) writes, one record per read:
+ * BamRead.toJson (read.d:768-830) plus '\n'.  Strings are escaped as writeStringJson does (only '"', '\\', '/' and bytes 8, 9, 10, 12, 13; every
+ * other byte is written as it is), qualities are an array of integers, f values and B:f elements print as %g with +-inf as +-1.0e+1024 and NaN
+ * as null.  Everything else is bdepth_run_view_text's: the selection and options, the order (positional regions one argument after the other,
+ * BDEPTH_VIEW_UNMAPPED for '*' in its place, n_unmapped 0), the pieces of whole lines handed to cb, BDEPTH_ERR_CALLBACK, the same
+ * BDEPTH_ERR_FORMAT refusals and messages, the several-rank join and its refusals.
+ * Timings: ms_inflate, ms_scan, ms_reduce (formatting kernels), ms_d2h (text copies), summed over the runs of a positional query. */
+int bdepth_run_view_json(bdepth_t* h, const bdepth_view_opts* opts, bdepth_text_cb cb, void* user);
 /* Scan records on the GPU; copy out up to cap rows of the columnar SoA (any pointer may be NULL). */
 int64_t bdepth_scan_to_host(bdepth_t* h, uint64_t cap, int32_t* ref_id, int32_t* pos, uint32_t* span, uint16_t* flag, uint8_t* mapq, uint16_t* n_cigar, uint64_t* rec_off);
 

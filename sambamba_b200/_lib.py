@@ -144,6 +144,7 @@ def load_library():
     L.bdepth_run_flagstat.argtypes = [vp, C.POINTER(FlagStat)]
     L.bdepth_run_view_count.argtypes = [vp, C.POINTER(ViewOpts), C.POINTER(C.c_uint64)]
     L.bdepth_run_view_text.argtypes = [vp, C.POINTER(ViewOpts), TEXT_CB, vp]
+    L.bdepth_run_view_json.argtypes = [vp, C.POINTER(ViewOpts), TEXT_CB, vp]
     _lib = L
     return L
 
@@ -154,7 +155,7 @@ EXPORTED_SYMBOLS = [
     "bdepth_n_samples", "bdepth_sample_name", "bdepth_set_filter", "bdepth_set_filter_query", "bdepth_set_min_baseq", "bdepth_set_fix_mates", "bdepth_set_combined", "bdepth_set_regions",
     "bdepth_set_shard", "bdepth_nccl_unique_id", "bdepth_plan_shards", "bdepth_plan_region_chunks", "bdepth_set_tuning", "bdepth_stage", "bdepth_run_resident", "bdepth_run_base", "bdepth_run_base_text",
     "bdepth_run_windows", "bdepth_run_regions", "bdepth_get_stats", "bdepth_ref_has_reads", "bdepth_inflate_to_host", "bdepth_scan_to_host", "bdepth_build_index",
-    "bdepth_run_flagstat", "bdepth_run_view_count", "bdepth_run_view_text",
+    "bdepth_run_flagstat", "bdepth_run_view_count", "bdepth_run_view_text", "bdepth_run_view_json",
 ]
 
 
@@ -428,10 +429,8 @@ class BDepth:
         self._ck(self.L.bdepth_run_view_count(self.h, C.byref(self._view_opts(num_filter, query, subsample, seed, bed, regions, n_unmapped)), C.byref(n)))
         return n.value
 
-    def run_view_text(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, sink=None):
-        """`sambamba view`: the SAM lines of the selected reads (no header).  The keywords are run_view_count's; `regions` may hold "*" entries,
-        each the region argument '*' in its place.  Returns the text, or hands each chunk to sink(bytes) and returns the number of bytes; a sink
-        that raises stops the run (BDepthError BDEPTH_ERR_CALLBACK, the sink's exception as its cause)."""
+    def _run_lines(self, entry, sink, opts):
+        """Calls entry(h, opts, cb, NULL) with a callback that gathers the text or streams it to sink; see run_view_text."""
         parts, total, err = [], [0], []
 
         def cb(_user, ptr, n):
@@ -443,12 +442,23 @@ class BDepth:
                 err.append(e)
                 return 1
         try:
-            self._ck(self.L.bdepth_run_view_text(self.h, C.byref(self._view_opts(num_filter, query, subsample, seed, bed, regions)), TEXT_CB(cb), None))
+            self._ck(entry(self.h, C.byref(opts), TEXT_CB(cb), None))
         except BDepthError as e:
             if err:
                 raise e from err[0]
             raise
         return total[0] if sink is not None else b"".join(parts)
+
+    def run_view_text(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, sink=None):
+        """`sambamba view`: the SAM lines of the selected reads (no header).  The keywords are run_view_count's; `regions` may hold "*" entries,
+        each the region argument '*' in its place.  Returns the text, or hands each chunk to sink(bytes) and returns the number of bytes; a sink
+        that raises stops the run (BDepthError BDEPTH_ERR_CALLBACK, the sink's exception as its cause)."""
+        return self._run_lines(self.L.bdepth_run_view_text, sink, self._view_opts(num_filter, query, subsample, seed, bed, regions))
+
+    def run_view_json(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, sink=None):
+        """`sambamba view -f json`: the JSON records of the selected reads, one per line.  Keywords, order, return value and sink as in
+        run_view_text."""
+        return self._run_lines(self.L.bdepth_run_view_json, sink, self._view_opts(num_filter, query, subsample, seed, bed, regions))
 
     def scan(self, cap):
         cols = dict(ref_id=np.zeros(cap, np.int32), pos=np.zeros(cap, np.int32), span=np.zeros(cap, np.uint32),

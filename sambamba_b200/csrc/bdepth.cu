@@ -95,6 +95,7 @@ constexpr uint32_t SHARD_EXTRA_BLOCKS = 8;
 constexpr uint32_t MATE_ZONE_BLOCKS = 64;       // -m on several ranks: blocks read behind the shard so that pairs cut by the boundary are seen whole
 
 enum RunMode { RUN_FULL = 0, RUN_INFLATE_ONLY = 1, RUN_SCAN_ONLY = 2, RUN_INDEX = 3, RUN_FLAGSTAT = 4, RUN_VIEW_COUNT = 5, RUN_VIEW_TEXT = 6 };
+enum TextFormat { TEXT_SAM, TEXT_JSON };      // the lines of RUN_VIEW_TEXT: BamRead.toSam or BamRead.toJson
 // Several ranks with NCCL: the collective of the current run that a rank owes its peers next.  A rank that stops with an error joins it with
 // a "failed" mark (abort_collectives), so that the others stop too instead of waiting for it.
 // BOUNDARY_TABLE: depth's all-gather in exchange_boundaries; SPARSE_DECISION: a sparse region query's all-reduce that tells whether every rank's
@@ -246,7 +247,8 @@ struct bdepth {
         bool pend[2] = {false, false}; size_t pend_len[2] = {0, 0}; int next = 0;
         uint64_t issued = 0;                           // bytes handed to the D2H in the current pipeline run
         float ms_fmt = 0, ms_d2h = 0;
-        SamTab tab{};                                  // the reference names on the device (ctl is set per sub-batch)
+        SamTab tab{};                                  // the reference names on the device, as the format prints them (ctl is set per sub-batch)
+        TextFormat fmt = TEXT_SAM;                     // which line view_text_sub formats: SAM (bdepth_run_view_text) or JSON (bdepth_run_view_json)
     } vt;
     // ---- several BAM files (bdepth_add_input; MultiBamReader, multireader.d:218-268): the additional files are whole handles that
     // only hold their input (file, BGZF members, header, index, shard / sparse plan); a run swaps them into this handle one after
@@ -738,7 +740,8 @@ int view_text_sub(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R
     SamTab t = V.tab; t.ctl = V.ctl.as<unsigned long long>();
     CK(cudaMemsetAsync(t.ctl, 0, 24, sm));
     CK(cudaEventRecord(h->ev[30], sm));
-    BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_sam_len)(soa, u0, R, own_from, h->vsel, t, len);
+    if (V.fmt == TEXT_JSON) BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_json_len)(soa, u0, R, own_from, h->vsel, t, len);
+    else BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_sam_len)(soa, u0, R, own_from, h->vsel, t, len);
     BD_LAUNCH(n_tiles, 256, 0, sm, k_sam_tile_sum)(len, R, tsum);
     BD_LAUNCH(1, 1024, 0, sm, k_text_scan)(tsum, n_tiles, toff, t.ctl);
     BD_LAUNCH(n_tiles, 256, 0, sm, k_sam_scan_apply)(len, R, toff, off);
@@ -772,7 +775,9 @@ int view_text_sub(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R
         const int s = V.next;
         int rc = view_text_deliver(h, s); if (rc) return rc;      // the slot's previous piece must be consumed before reuse
         CK(cudaEventRecord(h->ev[28 + s], sm));
-        BD_LAUNCH((unsigned)std::min<uint64_t>((r1 - r0 + 7) / 8, 8192), 256, 0, sm, k_sam_write)(soa.off, u0, r0, r1, len, off, t, V.slot[s].as<char>());
+        const unsigned grid = (unsigned)std::min<uint64_t>((r1 - r0 + 7) / 8, 8192);
+        if (V.fmt == TEXT_JSON) BD_LAUNCH(grid, 256, 0, sm, k_json_write)(soa.off, u0, r0, r1, len, off, t, V.slot[s].as<char>());
+        else BD_LAUNCH(grid, 256, 0, sm, k_sam_write)(soa.off, u0, r0, r1, len, off, t, V.slot[s].as<char>());
         CK(cudaGetLastError()); h->st.gpu_launches++;
         CK(cudaEventRecord(h->ev[24 + s], sm));
         CK(cudaStreamWaitEvent(h->s_d2h, h->ev[24 + s], 0));
@@ -2271,11 +2276,19 @@ int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* o, uint64_t* coun
     return 0;
 }
 
-// ---- view (SAM text) -------------------------------------------------------------------------------------------------------------
-// SamSerializer over view_main's reads (utils/view/alignmentrangeprocessor.d:97-106): the same selection as view -c, and the lines are written
-// inside the pipeline, sub-batch by sub-batch (view_text_sub).  Positional regions are joined as the reference joins them (view.d:308-366): one
-// pipeline run per region argument, in the order given, each staging only that region's BAI chunks ('*' scans the whole file).
-int bdepth_run_view_text(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb cb, void* user) {
+// ---- view (SAM and JSON text) ----------------------------------------------------------------------------------------------------
+// SamSerializer / JsonSerializer over view_main's reads (utils/view/alignmentrangeprocessor.d:97-106,149-158): the same selection as view -c, and
+// the lines are written inside the pipeline, sub-batch by sub-batch (view_text_sub).  Positional regions are joined as the reference joins them
+// (view.d:308-366): one pipeline run per region argument, in the order given, each staging only that region's BAI chunks ('*' scans the whole file).
+static std::string json_quote(const std::string& s) {      // writeStringJson (format.d:214-248), as json_line escapes on the device
+    std::string q = "\"";
+    for (unsigned char c : s) {
+        const char e = c == 8 ? 'b' : c == 9 ? 't' : c == 10 ? 'n' : c == 12 ? 'f' : c == 13 ? 'r' : (c == '"' || c == '/' || c == '\\') ? (char)c : 0;
+        if (e) { q += '\\'; q += e; } else q += (char)c;
+    }
+    return q + "\"";
+}
+static int run_view_lines(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb cb, void* user, TextFormat fmt) {
     if (!h) return BDEPTH_ERR_ARG;
     if (!o || (o->n_regions && !o->regions)) return fail(h, BDEPTH_ERR_ARG, "null argument");
     if (o->regions_from < BDEPTH_VIEW_ALL || o->regions_from > BDEPTH_VIEW_POSITIONAL) return fail(h, BDEPTH_ERR_ARG, "regions_from: %d", o->regions_from);
@@ -2288,14 +2301,14 @@ int bdepth_run_view_text(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb 
     auto& V = h->vt;
     {   // the reference names, once per call: offsets, then the names
         std::vector<uint32_t> noff(nref + 1, 0); std::string all;
-        for (size_t r = 0; r < nref; r++) { noff[r] = (uint32_t)all.size(); all += h->hdr.ref_names[r]; }
+        for (size_t r = 0; r < nref; r++) { noff[r] = (uint32_t)all.size(); all += fmt == TEXT_JSON ? json_quote(h->hdr.ref_names[r]) : h->hdr.ref_names[r]; }
         noff[nref] = (uint32_t)all.size();
         CK(V.names.ensure((nref + 1) * 4 + all.size() + 16));
         CK(cudaMemcpy(V.names.p, noff.data(), (nref + 1) * 4, cudaMemcpyHostToDevice));
         if (!all.empty()) CK(cudaMemcpy(V.names.as<uint8_t>() + (nref + 1) * 4, all.data(), all.size(), cudaMemcpyHostToDevice));
         V.tab = SamTab{(const char*)(V.names.as<uint8_t>() + (nref + 1) * 4), V.names.as<uint32_t>(), (int32_t)nref, nullptr};
     }
-    V.cb = cb; V.user = user; V.pend[0] = V.pend[1] = false; V.next = 0;
+    V.cb = cb; V.user = user; V.pend[0] = V.pend[1] = false; V.next = 0; V.fmt = fmt;
     auto one_run = [&](const bdepth_region* regs, size_t n, uint32_t n_star, bdepth_stats& acc) -> int {
         std::vector<bdepth_region> plan; bool empty = false;
         int r = view_setup(h, o, regs, n, n_star, plan, &empty); if (r) return r;
@@ -2333,6 +2346,8 @@ int bdepth_run_view_text(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb 
     h->st.ms_total_device = h->st.ms_h2d + h->st.ms_inflate + h->st.ms_scan + h->st.ms_reduce + h->st.ms_d2h;
     return 0;
 }
+int bdepth_run_view_text(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb cb, void* user) { return run_view_lines(h, o, cb, user, TEXT_SAM); }
+int bdepth_run_view_json(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb cb, void* user) { return run_view_lines(h, o, cb, user, TEXT_JSON); }
 
 int bdepth_ref_has_reads(const bdepth_t* h, int ref) {
     if (ref < 0 || (size_t)ref >= h->hdr.ref_len.size() || h->ref_has_host.empty()) return 0;

@@ -1837,4 +1837,197 @@ __global__ void __launch_bounds__(256, 1) k_sam_write(const int64_t* __restrict_
         if (len[r]) sam_line<true>(u + rec_off[r], t, out + (off[r] - base), lane);
 }
 
+// ---- sambamba view -f json: the JSON record of a read, BamRead.toJson (read.d:768-830) plus '\n' (chunkToFormat!'j',
+// alignmentrangeprocessor.d:66-82).  Built as sam_line is: a warp per record, lane 0 writes the fixed fields and the keys, the lanes share the
+// sequence, the qualities, the CIGAR ops, B array elements, the NUL search and the escaping of the name and of Z / H values; json_line<false>
+// measures the line and json_line<true> writes it.  The reference names in t arrive quoted and escaped (the host does it once per call).
+// Strings go through writeStringJson (format.d:214-248): only '"', '\\', '/' and bytes 8, 9, 10, 12, 13 are escaped; every other byte, control
+// bytes and bytes >= 0x80 included, is written as it is.  The refusals are sam_line's, for the same reasons.
+__device__ __forceinline__ char json_esc(uint8_t c) {      // the escape letter of c, 0 when c is written as it is (specialCharacterTable)
+    switch (c) {
+        case 8: return 'b'; case 9: return 't'; case 10: return 'n'; case 12: return 'f'; case 13: return 'r';
+        case '"': return '"'; case '/': return '/'; case '\\': return '\\';
+        default: return 0;
+    }
+}
+// the fixed text s at out + at when w; at advances in both passes
+template <int N>
+__device__ __forceinline__ void json_lit(char* out, uint32_t& at, bool w, const char (&s)[N]) { if (w) for (int i = 0; i < N - 1; i++) out[at + i] = s[i]; at += N - 1; }
+__device__ __forceinline__ void json_byte(char* out, uint32_t& at, bool w, uint8_t c) {
+    const char e = json_esc(c);
+    if (w) { if (e) { out[at] = '\\'; out[at + 1] = e; } else out[at] = (char)c; }
+    at += e ? 2u : 1u;
+}
+// the escaped bytes s[0, n), a byte per lane: its place is its index plus the escapes before it in the warp's 32 bytes (a ballot)
+template <bool WRITE>
+__device__ __forceinline__ void json_str(const uint8_t* s, uint32_t n, char* out, uint32_t& at, uint32_t lane) {
+    for (uint32_t b0 = 0; b0 < n; b0 += 32) {
+        const uint32_t i = b0 + lane;
+        const uint8_t c = i < n ? s[i] : 0; const char e = i < n ? json_esc(c) : 0;
+        const unsigned m = __ballot_sync(0xFFFFFFFFu, e != 0);
+        if (WRITE && i < n) { char* q = out + at + lane + __popc(m & ((1u << lane) - 1u)); if (e) { q[0] = '\\'; q[1] = e; } else q[0] = (char)c; }
+        at += min(32u, n - b0) + (uint32_t)__popc(m);
+    }
+}
+// writeFloatJson (format.d:196-212): finite values as %g, +-inf as +-1.0e+1024, every NaN as null.  At most 13 bytes.
+__device__ __forceinline__ uint32_t json_fmt_f(uint32_t bits, char* o) {
+    if (((bits >> 23) & 0xFFu) != 0xFFu) return sam_fmt_g(bits, o);
+    const char* s = (bits & 0x7FFFFFu) ? "null" : (bits >> 31) ? "-1.0e+1024" : "1.0e+1024";
+    uint32_t n = 0;
+    while (s[n]) { o[n] = s[n]; n++; }
+    return n;
+}
+
+template <bool WRITE>
+__device__ uint32_t json_line(const uint8_t* __restrict__ p, const SamTab& t, char* __restrict__ out, uint32_t lane) {
+    // p: the record's refID field; the record is the block_size bytes from there
+    const uint32_t bs = ldu32(p - 4);
+    const int32_t ref = (int32_t)ldu32(p), pos = (int32_t)ldu32(p + 4), l_seq = (int32_t)ldu32(p + 16), nref = (int32_t)ldu32(p + 20), npos = (int32_t)ldu32(p + 24), tlen = (int32_t)ldu32(p + 28);
+    const uint32_t bmn = ldu32(p + 8), fnc = ldu32(p + 12), l_name = bmn & 0xFFu, mapq = (bmn >> 8) & 0xFFu, flag = fnc >> 16, n_cig = fnc & 0xFFFFu;
+    const bool w0 = WRITE && lane == 0;
+    uint32_t err = 0;
+    if (ref < -1 || ref >= t.n_ref) err = SAM_ERR_REF;
+    else if (nref != ref && (nref < -1 || nref >= t.n_ref)) err = SAM_ERR_MATE_REF;
+    const uint64_t a0 = 32ull + l_name + 4ull * n_cig + ((uint64_t)(uint32_t)l_seq + 1) / 2 + (uint32_t)l_seq;
+    if (!err && (l_seq < 0 || a0 > bs)) err = SAM_ERR_OVERRUN;
+    if (err) { if (lane == 0) atomicMax(&t.ctl[2], (unsigned long long)err); return 0; }
+    uint32_t at = 0;
+    json_lit(out, at, w0, "{\"qname\":\"");
+    json_str<WRITE>(p + 32, l_name ? l_name - 1 : 0, out, at, lane);
+    json_lit(out, at, w0, "\",\"flag\":");
+    if (w0) put_dec(out + at, flag);
+    at += dec_digits(flag);
+    json_lit(out, at, w0, ",\"rname\":");
+    if (ref == -1) json_lit(out, at, w0, "\"*\"");
+    else { const uint32_t a = t.name_off[ref], n = t.name_off[ref + 1] - a; if (WRITE) for (uint32_t i = lane; i < n; i += 32) out[at + i] = t.names[a + i]; at += n; }
+    const int32_t pos1 = (int32_t)((uint32_t)pos + 1u), npos1 = (int32_t)((uint32_t)npos + 1u);      // D's int arithmetic wraps
+    json_lit(out, at, w0, ",\"pos\":");
+    if (w0) put_dec_i(out + at, pos1);
+    at += dec_len_i(pos1);
+    json_lit(out, at, w0, ",\"mapq\":");
+    if (w0) put_dec(out + at, mapq);
+    at += dec_digits(mapq);
+    json_lit(out, at, w0, ",\"cigar\":\"");
+    const uint8_t* cg = p + 32 + l_name;
+    if (!n_cig) json_lit(out, at, w0, "*");
+    for (uint32_t b0 = 0; b0 < n_cig; b0 += 32) {
+        const uint32_t i = b0 + lane; uint32_t c = 0, len = 0;
+        if (i < n_cig) { c = ldu32(cg + 4 * i); len = dec_digits(c >> 4) + 1; }
+        const uint32_t incl = sam_warp_incl(len, lane);
+        if (WRITE && i < n_cig) { char* q = put_dec(out + at + incl - len, c >> 4); *q = "MIDNSHP=X???????"[c & 15]; }
+        at += __shfl_sync(0xFFFFFFFFu, incl, 31);
+    }
+    json_lit(out, at, w0, "\",\"rnext\":");
+    if (nref == ref || nref == -1) { if (w0) { out[at] = '"'; out[at + 1] = nref == -1 ? '*' : '='; out[at + 2] = '"'; } at += 3; }
+    else { const uint32_t a = t.name_off[nref], n = t.name_off[nref + 1] - a; if (WRITE) for (uint32_t i = lane; i < n; i += 32) out[at + i] = t.names[a + i]; at += n; }
+    json_lit(out, at, w0, ",\"pnext\":");
+    if (w0) put_dec_i(out + at, npos1);
+    at += dec_len_i(npos1);
+    json_lit(out, at, w0, ",\"tlen\":");
+    if (w0) put_dec_i(out + at, tlen);
+    at += dec_len_i(tlen);
+    json_lit(out, at, w0, ",\"seq\":\"");
+    const uint8_t* sq = cg + 4 * n_cig; const uint8_t* qs = sq + ((uint32_t)l_seq + 1) / 2;
+    if (!l_seq) json_lit(out, at, w0, "*");
+    else { if (WRITE) for (uint32_t i = lane; i < (uint32_t)l_seq; i += 32) { const uint8_t b = sq[i >> 1]; out[at + i] = "=ACMGRSVTWYHKDBN"[(i & 1) ? (b & 15) : (b >> 4)]; } at += (uint32_t)l_seq; }
+    // the qualities as decimal integers, 0xFF included; element i is preceded by ',' when i > 0
+    json_lit(out, at, w0, "\",\"qual\":[");
+    for (uint32_t b0 = 0; b0 < (uint32_t)l_seq; b0 += 32) {
+        const uint32_t i = b0 + lane; uint32_t q = 0, len = 0;
+        if (i < (uint32_t)l_seq) { q = qs[i]; len = (q < 10u ? 1u : q < 100u ? 2u : 3u) + (i ? 1u : 0u); }
+        const uint32_t incl = sam_warp_incl(len, lane);
+        if (WRITE && i < (uint32_t)l_seq) { char* o = out + at + incl - len; if (i) *o++ = ','; put_dec(o, q); }
+        at += __shfl_sync(0xFFFFFFFFu, incl, 31);
+    }
+    json_lit(out, at, w0, "],\"tags\":{");
+    // tags: sam_line's walk, each a "key":value pair
+    const uint8_t* ax = p + a0; const uint32_t alen = bs - (uint32_t)a0;
+    uint32_t off = 0;
+    while (off + 1 < alen) {
+        if (off + 2 >= alen) { err = SAM_ERR_OVERRUN; break; }
+        const uint8_t ty = ax[off + 2];
+        if (off) json_lit(out, at, w0, ",");
+        json_lit(out, at, w0, "\"");
+        json_byte(out, at, w0, ax[off]); json_byte(out, at, w0, ax[off + 1]);
+        json_lit(out, at, w0, "\":");
+        off += 3;
+        if (ty == 'A') {
+            if (off + 1 > alen) { err = SAM_ERR_OVERRUN; break; }
+            json_lit(out, at, w0, "\""); json_byte(out, at, w0, ax[off]); json_lit(out, at, w0, "\"");
+            off += 1;
+        } else if (ty == 'c' || ty == 'C' || ty == 's' || ty == 'S' || ty == 'i' || ty == 'I') {
+            const uint32_t sz = sam_int_size(ty);
+            if (off + sz > alen) { err = SAM_ERR_OVERRUN; break; }
+            const int64_t v = sam_int(ty, ax + off);
+            if (w0) put_dec_i(out + at, v);
+            at += dec_len_i(v); off += sz;
+        } else if (ty == 'f') {
+            if (off + 4 > alen) { err = SAM_ERR_OVERRUN; break; }
+            char g[16]; const uint32_t n = json_fmt_f(ldu32(ax + off), g);
+            if (w0) for (uint32_t i = 0; i < n; i++) out[at + i] = g[i];
+            at += n; off += 4;
+        } else if (ty == 'Z' || ty == 'H') {
+            uint32_t nul = alen;                                // the warp looks for the NUL 32 bytes at a time
+            for (uint32_t b0 = off; b0 < alen; b0 += 32) {
+                const uint32_t i = b0 + lane;
+                const unsigned z = __ballot_sync(0xFFFFFFFFu, i < alen && ax[i] == 0);
+                if (z) { nul = b0 + (uint32_t)__ffs((int)z) - 1; break; }
+            }
+            if (nul == alen) { err = SAM_ERR_NO_NUL; break; }
+            json_lit(out, at, w0, "\"");
+            json_str<WRITE>(ax + off, nul - off, out, at, lane);
+            json_lit(out, at, w0, "\"");
+            off = nul + 1;
+        } else if (ty == 'B') {
+            if (off + 5 > alen) { err = SAM_ERR_OVERRUN; break; }
+            const uint8_t et = ax[off]; const uint32_t n = ldu32(ax + off + 1), sz = sam_int_size(et);
+            if (!sz) { err = SAM_ERR_B_TYPE; break; }
+            off += 5;
+            if ((uint64_t)n * sz > alen - off) { err = SAM_ERR_OVERRUN; break; }
+            json_lit(out, at, w0, "[");
+            for (uint32_t b0 = 0; b0 < n; b0 += 32) {           // element i is preceded by ',' when i > 0 (writeArrayJson, format.d:256-270)
+                const uint32_t i = b0 + lane; uint32_t len = 0; char g[16]; int64_t v = 0;
+                if (i < n) {
+                    if (et == 'f') len = json_fmt_f(ldu32(ax + off + 4 * i), g);
+                    else { v = sam_int(et, ax + off + sz * i); len = dec_len_i(v); }
+                    len += i ? 1u : 0u;
+                }
+                const uint32_t incl = sam_warp_incl(len, lane);
+                if (WRITE && i < n) {
+                    char* q = out + at + incl - len;
+                    if (i) *q++ = ',';
+                    if (et == 'f') { for (uint32_t k = 0; k < len - (i ? 1u : 0u); k++) q[k] = g[k]; }
+                    else put_dec_i(q, v);
+                }
+                at += __shfl_sync(0xFFFFFFFFu, incl, 31);
+            }
+            json_lit(out, at, w0, "]");
+            off += n * sz;
+        } else { err = SAM_ERR_TAG_TYPE; break; }
+    }
+    if (err) { if (lane == 0) atomicMax(&t.ctl[2], (unsigned long long)err); return 0; }
+    json_lit(out, at, w0, "}}\n");
+    return at;
+}
+
+// k_sam_len and k_sam_write for JSON records: the same launch shapes, the same scan, cut and slots between them
+__global__ void __launch_bounds__(256, 1) k_json_len(RecordSoA soa, const uint8_t* __restrict__ u, uint32_t R, int64_t own_from, ViewSel vs, SamTab t, uint32_t* __restrict__ len) {
+    const uint32_t lane = threadIdx.x & 31, nw = gridDim.x * (blockDim.x >> 5);
+    uint32_t mx = 0;
+    for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < R; r += nw) {
+        uint32_t n = 0;
+        if (view_select(soa, u, r, own_from, vs)) n = json_line<false>(u + soa.off[r], t, nullptr, lane);
+        if (lane == 0) len[r] = n;
+        mx = n > mx ? n : mx;
+    }
+    if (lane == 0 && mx) atomicMax(&t.ctl[1], (unsigned long long)mx);
+}
+__global__ void __launch_bounds__(256, 1) k_json_write(const int64_t* __restrict__ rec_off, const uint8_t* __restrict__ u, uint32_t r0, uint32_t r1, const uint32_t* __restrict__ len,
+                                                    const unsigned long long* __restrict__ off, SamTab t, char* __restrict__ out) {
+    const uint32_t lane = threadIdx.x & 31, nw = gridDim.x * (blockDim.x >> 5);
+    const unsigned long long base = off[r0];
+    for (uint32_t r = r0 + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5); r < r1; r += nw)
+        if (len[r]) json_line<true>(u + rec_off[r], t, out + (off[r] - base), lane);
+}
+
 }  // namespace bdk

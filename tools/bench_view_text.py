@@ -23,7 +23,10 @@ for d in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tools")):
     sys.path.insert(0, d)
 
 
-def timed(h, warmup, steps, bed=None):
+ENTRY = {"sam": "bdepth_run_view_text", "json": "bdepth_run_view_json"}
+
+
+def timed(h, warmup, steps, bed=None, fmt="sam"):
     import sambamba_b200._lib as SL
     o = SL.ViewOpts()
     arr = (SL.Region * max(len(bed or []), 1))(*[SL.Region(*r) for r in bed or []])
@@ -37,7 +40,7 @@ def timed(h, warmup, steps, bed=None):
     def hashing(_user, ptr, n):
         sha.update(C.string_at(ptr, n))
         return 0
-    run = lambda cb: h._ck(h.L.bdepth_run_view_text(h.h, C.byref(o), cb, None))      # noqa: E731
+    run = lambda cb: h._ck(getattr(h.L, ENTRY[fmt])(h.h, C.byref(o), cb, None))      # noqa: E731
     cb = SL.TEXT_CB(discard)
     for _ in range(warmup):
         run(cb)
@@ -51,19 +54,20 @@ def timed(h, warmup, steps, bed=None):
     run(SL.TEXT_CB(hashing))                                 # verification, after the timed region
     med = lambda k: round(statistics.median(s[k] for s in st), 3)      # noqa: E731
     return {"host_ms_median": round(statistics.median(host), 3), "host_ms_min": round(min(host), 3), "host_ms_max": round(max(host), 3),
-            "k1_inflate_ms_median": med("ms_inflate"), "k2_scan_ms_median": med("ms_scan"), "sam_kernels_ms_median": med("ms_reduce"),
+            "k1_inflate_ms_median": med("ms_inflate"), "k2_scan_ms_median": med("ms_scan"), fmt + "_kernels_ms_median": med("ms_reduce"),
             "text_d2h_ms_median": med("ms_d2h"), "file_bytes": st[-1]["file_bytes"], "text_bytes": nbytes[0],
             "text_gb_per_s": round(nbytes[0] / 1e9 / (statistics.median(host) / 1e3), 3), "sha256": sha.hexdigest()}
 
 
-def main():
+def main(fmt="sam"):
+    """fmt: "sam" (bdepth_run_view_text) or "json" (bdepth_run_view_json, for bench_view_json.py)."""
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     a = ap.parse_args()
     import bench
     import sambamba_b200 as sb
-    import view_text_common as vt
+    vt = __import__("view_json_common" if fmt == "json" else "view_text_common")      # the oracle's SHA-256 of the same text
     from bench_flagstat import card
     info = card()
     path = bench.ensure_workload(1, bench.READS_PER_UNIT)
@@ -72,17 +76,17 @@ def main():
         L, name = h.refs[0][1], h.refs[0][0]
         bed = [(0, L // 2, L // 2 + L // 100)]
         h.stage()
-        resident = timed(h, a.warmup, a.steps)
+        resident = timed(h, a.warmup, a.steps, fmt=fmt)
     with sb.BDepth(path) as h:
-        sparse = timed(h, a.warmup, a.steps, bed=bed)
+        sparse = timed(h, a.warmup, a.steps, bed=bed, fmt=fmt)
     img, keep = bench.pinned_file(path)
     with sb.BDepth(memory=img) as h:
-        e2e = timed(h, a.warmup, a.steps)
+        e2e = timed(h, a.warmup, a.steps, fmt=fmt)
     del keep
     want = vt.oracle_sha256(path)
     want_s = vt.oracle_sha256(path, bed="%s\t%d\t%d\n" % (name, bed[0][1], bed[0][2]))
     verified = (resident["sha256"], resident["text_bytes"]) == (e2e["sha256"], e2e["text_bytes"]) == want and (sparse["sha256"], sparse["text_bytes"]) == want_s
-    print(json.dumps({"metric": "bam_gb_per_s_view_text", "unit": "GB/s", "card": info, "workload": f"{os.path.basename(path)}: {bench.READS_PER_UNIT:,} reads, seed 20",
+    print(json.dumps({"metric": "bam_gb_per_s_view_" + ("json" if fmt == "json" else "text"), "unit": "GB/s", "card": info, "workload": f"{os.path.basename(path)}: {bench.READS_PER_UNIT:,} reads, seed 20",
                       "value": round(gb / (resident["host_ms_median"] / 1e3), 3), "resident": resident, "e2e": dict(e2e, value=round(gb / (e2e["host_ms_median"] / 1e3), 3)),
                       "sparse": dict(sparse, region="%s:%d-%d" % (name, bed[0][1] + 1, bed[0][2])), "oracle": [want, want_s], "verified": verified}))
     return 0 if verified else 1

@@ -1,4 +1,4 @@
-/* view_count_oracle.c -- CPU restatement of `sambamba view -c` and of `sambamba view`'s SAM lines (TEST INFRASTRUCTURE: the checker the GPU
+/* view_count_oracle.c -- CPU restatement of `sambamba view -c` and of `sambamba view`'s SAM lines and JSON records (TEST INFRASTRUCTURE: the checker the GPU
  * count and text are compared with).
  *
  * What is restated (sambamba/view.d:265-379), record by record, without shortcuts:
@@ -17,11 +17,13 @@
  * (alignmentrangeprocessor.d:72-75), with the tag values of tagvalue.d:468-504 and floats through snprintf("%g", (double)f) as
  * bio/core/utils/format.d:92-134 does.  Where the reference throws or indexes out of bounds (an unknown tag type, a tag running past the record,
  * a Z / H value without its NUL, a reference ID outside [-1, n_ref) that is printed), the text entry point returns an error.
- * Library: view_count_oracle(), view_text_oracle(), view_text_oracle_free(), view_count_oracle_hash(), view_count_oracle_error().  With
- * -DORACLE_MAIN also a CLI:
- *   view_count_oracle view [-c] [--num-filter=I1/I2] [-s FRAC] [--subsampling-seed=SEED] [-L BED] in.bam [region ...]
- * which prints the count as `sambamba view -c` does, or without -c the SAM lines (no header), or "sambamba-view: <msg>" and exit code 1 for the
- * errors it restates. */
+ * The JSON record of `view -f json` is a literal C statement of BamRead.toJson (read.d:768-830) plus '\n' with BioD's writers: writeStringJson and
+ * its escape table, writeFloatJson (%g, +-1.0e+1024 for +-inf, null for NaN) and itoa (format.d:66-87,196-270); its refusals are the SAM line's.
+ * Library: view_count_oracle(), view_text_oracle(), view_json_oracle(), view_text_oracle_free(), view_count_oracle_hash(),
+ * view_count_oracle_error().  With -DORACLE_MAIN also a CLI:
+ *   view_count_oracle view [-c] [-f sam|json] [--num-filter=I1/I2] [-s FRAC] [--subsampling-seed=SEED] [-L BED] in.bam [region ...]
+ * which prints the count as `sambamba view -c` does, or without -c the SAM lines or JSON records (no header), or "sambamba-view: <msg>" and exit
+ * code 1 for the errors it restates. */
 #include <ctype.h>
 #include <errno.h>
 #include <math.h>
@@ -103,7 +105,7 @@ uint64_t view_count_oracle_hash(const uint8_t* name, size_t len, uint64_t seed) 
 typedef struct { uint32_t ref, start, end; } Reg;
 
 /* Where selected reads go: counted, or formatted as SAM lines into a growing buffer. */
-typedef struct { int text; uint64_t cnt; char* buf; size_t len, cap; int err; } Out;
+typedef struct { int text, json; uint64_t cnt; char* buf; size_t len, cap; int err; } Out;
 static void out_put(Out* o, const void* s, size_t n) {
     if (o->len + n > o->cap) { o->cap = (o->len + n) * 2 + 4096; o->buf = realloc(o->buf, o->cap); }
     memcpy(o->buf + o->len, s, n); o->len += n;
@@ -184,9 +186,121 @@ static int sam_line(const Bam* b, const Rec* x, Out* o) {
     out_str(o, "\n");
     return 0;
 }
+
+/* ---- BamRead.toJson (read.d:768-830) with BioD's JSON writers (bio/core/utils/format.d) */
+static const char specialCharacterTable[256] = {                            /* format.d:221-240: the escape letter, 0 = written as it is */
+    ['\b'] = 'b', ['\t'] = 't', ['\n'] = 'n', ['\f'] = 'f', ['\r'] = 'r', ['"'] = '"', ['/'] = '/', ['\\'] = '\\' };
+static void writeStringJson(Out* o, const uint8_t* s, size_t n) {          /* format.d:242-254 */
+    out_str(o, "\"");
+    for (size_t i = 0; i < n; i++) {
+        const char sc = specialCharacterTable[s[i]];
+        if (sc == 0) out_put(o, s + i, 1);
+        else { out_str(o, "\\"); out_put(o, &sc, 1); }
+    }
+    out_str(o, "\"");
+}
+/* itoa (format.d:66-87): digits of the magnitude, reversed.  BioD negates a signed value in int before widening it to ulong, so at INT32_MIN it
+ * would print -18446744071562067968; this restatement prints -2147483648 as the SAM lines do (a stated deviation, DESIGN.md section 8). */
+static void itoa_json(Out* o, long long value) {
+    char str[32], *wstr = str;
+    unsigned long long uvalue = value < 0 ? (unsigned long long)(-value) : (unsigned long long)value;
+    do { *wstr++ = (char)(48 + (uvalue % 10)); } while (uvalue /= 10);
+    if (value < 0) *wstr++ = '-';
+    for (char *b = str, *e = wstr - 1, t; e > b; b++, e--) { t = *e; *e = *b; *b = t; }
+    out_put(o, str, (size_t)(wstr - str));
+}
+static void writeFloatJson(Out* o, float value) {                            /* format.d:196-212 */
+    if (isfinite(value)) out_g(o, value);
+    else if (value == INFINITY) out_str(o, "1.0e+1024");
+    else if (value == -INFINITY) out_str(o, "-1.0e+1024");
+    else out_str(o, "null");
+}
+static void json_val(Out* o, uint8_t t, const uint8_t* e) {                 /* one integer or float value (tagvalue.d:515-538) */
+    switch (t) {
+        case 'c': itoa_json(o, (int8_t)e[0]); break;
+        case 'C': itoa_json(o, e[0]); break;
+        case 's': itoa_json(o, (int16_t)(e[0] | (e[1] << 8))); break;
+        case 'S': itoa_json(o, (uint16_t)(e[0] | (e[1] << 8))); break;
+        case 'i': itoa_json(o, (int32_t)rd32(e)); break;
+        case 'I': itoa_json(o, rd32(e)); break;
+        default: { uint32_t w = rd32(e); float f; memcpy(&f, &w, 4); writeFloatJson(o, f); }
+    }
+}
+static int json_line(const Bam* b, const Rec* x, Out* o) {
+    const uint8_t* p = x->p; const uint32_t bs = x->bs;
+    const int32_t ref = (int32_t)rd32(p), pos = (int32_t)rd32(p + 4), l_seq = (int32_t)rd32(p + 16), nref = (int32_t)rd32(p + 20), npos = (int32_t)rd32(p + 24), tlen = (int32_t)rd32(p + 28);
+    const uint32_t bmn = rd32(p + 8), fnc = rd32(p + 12), l_name = bmn & 0xFF, mapq = (bmn >> 8) & 0xFF, flag = fnc >> 16, n_cig = fnc & 0xFFFF;
+    if (ref < -1 || ref >= b->n_ref) return sam_fail(o, "reference ID out of range");
+    if (nref != ref && (nref < -1 || nref >= b->n_ref)) return sam_fail(o, "mate reference ID out of range");
+    const uint64_t a0 = 32ull + l_name + 4ull * n_cig + ((uint64_t)(uint32_t)l_seq + 1) / 2 + (uint32_t)l_seq;
+    if (l_seq < 0 || a0 > bs) return sam_fail(o, "record fields run past block_size");
+    out_str(o, "{\"qname\":"); writeStringJson(o, p + 32, l_name ? l_name - 1 : 0);
+    out_str(o, ",\"flag\":"); itoa_json(o, flag);
+    out_str(o, ",\"rname\":");
+    if (ref == -1) out_str(o, "\"*\""); else writeStringJson(o, (const uint8_t*)b->names[ref], strlen(b->names[ref]));
+    out_str(o, ",\"pos\":"); itoa_json(o, (int32_t)((uint32_t)pos + 1u));        /* position + 1 in D's int: wraps */
+    out_str(o, ",\"mapq\":"); itoa_json(o, mapq);
+    out_str(o, ",\"cigar\":\"");
+    const uint8_t* cg = p + 32 + l_name;
+    if (!n_cig) out_str(o, "*");
+    for (uint32_t i = 0; i < n_cig; i++) { uint32_t c = rd32(cg + 4 * i); itoa_json(o, c >> 4); out_put(o, &"MIDNSHP=X???????"[c & 15], 1); }
+    out_str(o, "\"");
+    out_str(o, ",\"rnext\":");
+    if (nref == ref) out_str(o, nref == -1 ? "\"*\"" : "\"=\"");
+    else if (nref == -1) out_str(o, "\"*\"");
+    else writeStringJson(o, (const uint8_t*)b->names[nref], strlen(b->names[nref]));
+    out_str(o, ",\"pnext\":"); itoa_json(o, (int32_t)((uint32_t)npos + 1u));
+    out_str(o, ",\"tlen\":"); itoa_json(o, tlen);
+    out_str(o, ",\"seq\":\"");
+    const uint8_t* sq = cg + 4 * n_cig; const uint8_t* qs = sq + ((uint32_t)l_seq + 1) / 2;
+    if (l_seq == 0) out_str(o, "*");
+    for (int32_t i = 0; i < l_seq; i++) out_put(o, &"=ACMGRSVTWYHKDBN"[(i & 1) ? (sq[i >> 1] & 15) : (sq[i >> 1] >> 4)], 1);
+    out_str(o, "\"");
+    out_str(o, ",\"qual\":");                                                /* writeArrayJson (format.d:256-270) of the raw bytes */
+    if (l_seq == 0) out_str(o, "[]");
+    else { out_str(o, "["); for (int32_t i = 0; i < l_seq; i++) { if (i) out_str(o, ","); itoa_json(o, qs[i]); } out_str(o, "]"); }
+    out_str(o, ",\"tags\":{");
+    const uint8_t* ax = p + a0; const size_t alen = bs - a0;
+    size_t off = 0; int not_first = 0;
+    while (off + 1 < alen) {                                                /* opApply, read.d:1173-1186 */
+        if (not_first) out_str(o, ",");
+        writeStringJson(o, ax + off, 2); out_str(o, ":");
+        off += 2;
+        if (off >= alen) return sam_fail(o, "tag runs past the record");
+        const uint8_t t = ax[off++];
+        const uint32_t sz = val_size(t);
+        if (t == 'A') {
+            if (off + 1 > alen) return sam_fail(o, "tag runs past the record");
+            writeStringJson(o, ax + off, 1); off += 1;                       /* writeCharJson */
+        } else if (sz) {
+            if (off + sz > alen) return sam_fail(o, "tag runs past the record");
+            json_val(o, t, ax + off); off += sz;
+        } else if (t == 'Z' || t == 'H') {
+            const uint8_t* z = memchr(ax + off, 0, alen - off);
+            if (!z) return sam_fail(o, "Z or H value without its NUL");
+            writeStringJson(o, ax + off, (size_t)(z - (ax + off))); off = (size_t)(z - ax) + 1;
+        } else if (t == 'B') {
+            if (off + 5 > alen) return sam_fail(o, "B array runs past the record");
+            const uint8_t et = ax[off]; const uint32_t n = rd32(ax + off + 1), esz = val_size(et); off += 5;
+            if (!esz) return sam_fail(o, "unknown B array element type");
+            if ((uint64_t)n * esz > alen - off) return sam_fail(o, "B array runs past the record");
+            if (n == 0) out_str(o, "[]");
+            else {
+                out_str(o, "[");
+                for (uint32_t i = 0; i + 1 < n; i++) { json_val(o, et, ax + off + (size_t)esz * i); out_str(o, ","); }
+                json_val(o, et, ax + off + (size_t)esz * (n - 1)); out_str(o, "]");
+            }
+            off += (size_t)n * esz;
+        } else return sam_fail(o, "unknown tag type");
+        not_first = 1;
+    }
+    out_str(o, "}}\n");
+    return 0;
+}
+
 static void emit(const Bam* b, const Rec* x, Out* o) {
     if (!o->text) { o->cnt++; return; }
-    if (!o->err) sam_line(b, x, o);
+    if (!o->err) (o->json ? json_line : sam_line)(b, x, o);
 }
 
 /* BamReadFilter (randomaccessmanager.d:366-462): number of records of rec[0..n) the state machine yields for the sorted, non-overlapping regions. */
@@ -281,17 +395,26 @@ int view_count_oracle(const char* path, unsigned flag_set, unsigned flag_unset, 
     return rc;
 }
 
-/* The SAM lines `sambamba view` prints after the header, in the order of its joined stream; *text is freed with view_text_oracle_free(). */
-int view_text_oracle(const char* path, unsigned flag_set, unsigned flag_unset, int subsample, uint64_t threshold, uint64_t seed,
-                     int mode, const uint32_t* regs, size_t nreg, char** text, size_t* len) {
+static int text_oracle(const char* path, unsigned flag_set, unsigned flag_unset, int subsample, uint64_t threshold, uint64_t seed,
+                       int mode, const uint32_t* regs, size_t nreg, int json, char** text, size_t* len) {
     Bam b; g_err[0] = 0;
     if (bam_load(path, &b)) { bam_free(&b); return -1; }
-    Out o = {0}; o.text = 1;
+    Out o = {0}; o.text = 1; o.json = json;
     const int rc = view_stream(&b, flag_set, flag_unset, subsample, threshold, seed, mode, regs, nreg, 0, &o);
     bam_free(&b);
     if (rc) { free(o.buf); return -1; }
     *text = o.buf; *len = o.len;
     return 0;
+}
+/* The SAM lines `sambamba view` prints after the header, in the order of its joined stream; *text is freed with view_text_oracle_free(). */
+int view_text_oracle(const char* path, unsigned flag_set, unsigned flag_unset, int subsample, uint64_t threshold, uint64_t seed,
+                     int mode, const uint32_t* regs, size_t nreg, char** text, size_t* len) {
+    return text_oracle(path, flag_set, flag_unset, subsample, threshold, seed, mode, regs, nreg, 0, text, len);
+}
+/* The records `sambamba view -f json` prints, in the same order; *text is freed with view_text_oracle_free(). */
+int view_json_oracle(const char* path, unsigned flag_set, unsigned flag_unset, int subsample, uint64_t threshold, uint64_t seed,
+                     int mode, const uint32_t* regs, size_t nreg, char** text, size_t* len) {
+    return text_oracle(path, flag_set, flag_unset, subsample, threshold, seed, mode, regs, nreg, 1, text, len);
 }
 void view_text_oracle_free(char* text) { free(text); }
 
@@ -326,7 +449,7 @@ static void parse_region(const char* s, char* ref, size_t cap, uint32_t* beg, ui
 }
 int main(int argc, char** argv) {
     if (argc < 2 || strcmp(argv[1], "view")) { fprintf(stderr, "usage: view_count_oracle view [-c] [options] in.bam [region ...]\n"); return 1; }
-    unsigned long long fs = 0, fu = 0, seed = 0; double frac = NAN; const char* bed = NULL; int count = 0;
+    unsigned long long fs = 0, fu = 0, seed = 0; double frac = NAN; const char* bed = NULL; int count = 0, json = 0;
     const char* pos_args[4096]; int npos = 0;
     for (int i = 2; i < argc; i++) {
         const char* a = argv[i];
@@ -339,6 +462,11 @@ int main(int argc, char** argv) {
         } else if (!strcmp(a, "-s") && i + 1 < argc) frac = strtod(argv[++i], NULL);
         else if (!strncmp(a, "--subsampling-seed=", 19)) { if (conv_u(a + 19, 0xFFFFFFFFFFFFFFF0ull, "ulong", &seed)) return 1; }
         else if (!strcmp(a, "-L") && i + 1 < argc) bed = argv[++i];
+        else if (!strcmp(a, "-f") && i + 1 < argc) {
+            const char* f = argv[++i];
+            if (strcmp(f, "sam") && strcmp(f, "json")) return die("output format must be sam or json here");
+            json = !strcmp(f, "json");
+        }
         else if (npos < 4096) pos_args[npos++] = a;
     }
     if (npos < 1) { fprintf(stderr, "usage: view_count_oracle view [-c] [options] in.bam [region ...]\n"); return 1; }
@@ -392,7 +520,7 @@ int main(int argc, char** argv) {
     if (!count) {
         if (mode == 2 && !n) mode = 0;
         char* text = NULL; size_t len = 0;
-        if (view_text_oracle(pos_args[0], (unsigned)fs, (unsigned)fu, sub, thr, seed, mode, regs, n, &text, &len)) { free(regs); return die(g_err); }
+        if (text_oracle(pos_args[0], (unsigned)fs, (unsigned)fu, sub, thr, seed, mode, regs, n, json, &text, &len)) { free(regs); return die(g_err); }
         fwrite(text, 1, len, stdout); free(text); free(regs);
         return 0;
     }
