@@ -27,6 +27,8 @@
  *     (BamRead.toSam per read)           utils/view/alignmentrangeprocessor.d:97-106
  *   JsonSerializer over view_main's     sambamba/view.d:265-379,        bdepth_run_view_json (`sambamba view -f json`)
  *     reads (BamRead.toJson per read)    utils/view/alignmentrangeprocessor.d:149-158
+ *   ValidAlignmentFilter (isValid)       utils/common/filtering.d:78-83, bdepth_view_opts.valid (`view -v`, for the three
+ *                                        bio/std/hts/bam/validation/alignment.d   view entry points above)
  *
  * Conventions: every entry returns 0 on success or a negative bdepth_status; the message is
  * available through bdepth_last_error().  No exception crosses the boundary.  There is no CPU
@@ -269,7 +271,17 @@ typedef struct {
     const bdepth_region* regions;        /* -L: any order, merged as parseBed merges (bed.d:43-58); positional: one query each, start < end */
     size_t n_regions;
     uint32_t n_unmapped;                 /* positional: how many of the region arguments were '*' (unmappedReads, reader.d:370-391) */
+    int valid;                           /* -v (ValidAlignmentFilter, filtering.d:78-83): keep only reads BioD's isValid accepts (see below); 0 keeps all */
 } bdepth_view_opts;
+/* valid != 0: after -s and before --num-filter and -F (view.d:265-289), a read is dropped unless isValid (BioD/bio/std/hts/bam/validation/
+ * alignment.d:138-562) accepts it: a name of 1-255 bytes in [!-~] without '@'; a position in [-1, 2^29 - 2]; qualities all 0xFF or all in [0, 93];
+ * a CIGAR (as written; empty passes) with H only first or last, S only first or last once the end Hs are dropped (both only checked beyond 2 ops),
+ * and M/I/S/=/X lengths summing to l_seq (when l_seq > 0, in 32-bit wrapping arithmetic); tags that are well-formed (H: non-empty hex, A: [!-~],
+ * Z: non-empty [ -~]), predefined keys of their type (integer, Z, FZ as B:S), CQ E2 OQ Q2 U2 without spaces, BQ and E2 of length l_seq, MD of
+ * the grammar ^[0-9]+(([A-Z]|\^[A-Z]+)[0-9]+)*$, and no key twice.  A read that passes the first four checks has all its tags walked, and a
+ * walk that fails (an unknown tag or B element type, a Z / H value without its NUL, a tag running past the record) is BDEPTH_ERR_FORMAT with
+ * the SAM lines' messages -- if the validator reaches the read: -s keeps it and it is in the reference's stream (every record without regions
+ * and for -L on an unsorted file; otherwise only reads in a region, '*' included).  --num-filter and -F do not spare it.  Time: ms_reduce. */
 /* The number `sambamba view -c` prints: ReadCounter (utils/view/alignmentrangeprocessor.d:42-50) over the reads view_main selects, as one call --
  * options and printing stay with the host.  K1 inflate and the K2 record scan as in every run, then one thread per record (k_view_count).
  *   - BDEPTH_VIEW_ALL: every record of the file; neither SO:coordinate nor a .bai is needed on one GPU.

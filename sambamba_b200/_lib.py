@@ -60,7 +60,8 @@ class FlagStat(C.Structure):
 
 class ViewOpts(C.Structure):
     _fields_ = [("flag_set", C.c_uint16), ("flag_unset", C.c_uint16), ("query", C.c_char_p), ("subsample", C.c_int), ("subsample_threshold", C.c_uint64),
-                ("subsampling_seed", C.c_uint64), ("regions_from", C.c_int), ("regions", C.POINTER(Region)), ("n_regions", C.c_size_t), ("n_unmapped", C.c_uint32)]
+                ("subsampling_seed", C.c_uint64), ("regions_from", C.c_int), ("regions", C.POINTER(Region)), ("n_regions", C.c_size_t), ("n_unmapped", C.c_uint32),
+                ("valid", C.c_int)]
 
 
 def subsample_threshold(frac):
@@ -410,8 +411,9 @@ class BDepth:
         return fs.as_dict()
 
     @staticmethod
-    def _view_opts(num_filter, query, subsample, seed, bed, regions, n_unmapped=0):
+    def _view_opts(num_filter, query, subsample, seed, bed, regions, n_unmapped=0, valid=False):
         o = ViewOpts()
+        o.valid = 1 if valid else 0
         o.flag_set, o.flag_unset = num_filter
         o.query = query.encode() if query is not None else None
         if subsample is not None:
@@ -422,11 +424,11 @@ class BDepth:
         o.regions, o.n_regions, o.n_unmapped = o._arr, len(rg), n_unmapped
         return o
 
-    def run_view_count(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, n_unmapped=0):
+    def run_view_count(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, n_unmapped=0, valid=False):
         """`sambamba view -c`: the number of selected reads.  num_filter = (i1, i2); subsample = fraction (with `seed`); bed = [(ref, beg, end)]
-        as -L; regions = [(ref, beg, end)] positional queries, plus n_unmapped '*' queries."""
+        as -L; regions = [(ref, beg, end)] positional queries, plus n_unmapped '*' queries; valid = -v (bdepth_view_opts.valid)."""
         n = C.c_uint64()
-        self._ck(self.L.bdepth_run_view_count(self.h, C.byref(self._view_opts(num_filter, query, subsample, seed, bed, regions, n_unmapped)), C.byref(n)))
+        self._ck(self.L.bdepth_run_view_count(self.h, C.byref(self._view_opts(num_filter, query, subsample, seed, bed, regions, n_unmapped, valid)), C.byref(n)))
         return n.value
 
     def _run_lines(self, entry, sink, opts):
@@ -449,16 +451,16 @@ class BDepth:
             raise
         return total[0] if sink is not None else b"".join(parts)
 
-    def run_view_text(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, sink=None):
+    def run_view_text(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, sink=None, valid=False):
         """`sambamba view`: the SAM lines of the selected reads (no header).  The keywords are run_view_count's; `regions` may hold "*" entries,
         each the region argument '*' in its place.  Returns the text, or hands each chunk to sink(bytes) and returns the number of bytes; a sink
         that raises stops the run (BDepthError BDEPTH_ERR_CALLBACK, the sink's exception as its cause)."""
-        return self._run_lines(self.L.bdepth_run_view_text, sink, self._view_opts(num_filter, query, subsample, seed, bed, regions))
+        return self._run_lines(self.L.bdepth_run_view_text, sink, self._view_opts(num_filter, query, subsample, seed, bed, regions, valid=valid))
 
-    def run_view_json(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, sink=None):
+    def run_view_json(self, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, sink=None, valid=False):
         """`sambamba view -f json`: the JSON records of the selected reads, one per line.  Keywords, order, return value and sink as in
         run_view_text."""
-        return self._run_lines(self.L.bdepth_run_view_json, sink, self._view_opts(num_filter, query, subsample, seed, bed, regions))
+        return self._run_lines(self.L.bdepth_run_view_json, sink, self._view_opts(num_filter, query, subsample, seed, bed, regions, valid=valid))
 
     def scan(self, cap):
         cols = dict(ref_id=np.zeros(cap, np.int32), pos=np.zeros(cap, np.int32), span=np.zeros(cap, np.uint32),

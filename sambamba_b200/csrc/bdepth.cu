@@ -237,7 +237,10 @@ struct bdepth {
     // ---- flagstat (bdepth_run_flagstat): the counters of k_flagstat plus one word that marks a failed rank in the all-reduce, and their host copy
     DevBuf fs; uint64_t fs_host[FS_WORDS + 1] = {};
     // ---- view -c (bdepth_run_view_count): the selection of the current run, its device tables, the count plus a "failed rank" word and their host copy
+    // (vc holds a third word after them: the highest SAM_ERR_* code -v met, outside the all-reduce)
     ViewSel vsel{}; DevBuf vc, vc_reg, vc_prog; uint64_t vc_host[2] = {};
+    // ---- view -v: k_view_valid's status of each record of the sub-batch
+    bool view_valid = false; DevBuf vv;
     // ---- view's SAM lines (bdepth_run_view_text): per sub-batch the line lengths, their offsets and the piece cuts; two text slots on the device
     // and their pinned host copies (one is handed to the callback while the next piece is written and copied); timings of the run
     struct ViewText {
@@ -730,6 +733,14 @@ int view_text_deliver(bdepth* h, int slot) {
     return 0;
 }
 int view_text_flush(bdepth* h) { int rc = view_text_deliver(h, h->vt.next); if (!rc) rc = view_text_deliver(h, h->vt.next ^ 1); return rc; }
+// view -v: k_view_valid over the sub-batch's R records, and vs (the run's selection) pointed at its statuses, refusals going to *err
+int launch_view_valid(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R, int64_t own_from, unsigned long long* err, ViewSel& vs) {
+    CK(h->vv.ensure(R));
+    BD_LAUNCH((unsigned)std::min<uint64_t>((R + VV_WARPS - 1) / VV_WARPS, 8192), VV_WARPS * 32, 0, h->s_main, k_view_valid)(soa, u0, R, own_from, h->vv.as<uint8_t>());
+    CK(cudaGetLastError()); h->st.gpu_launches++;
+    vs.vstat = h->vv.as<uint8_t>(); vs.verr = err;
+    return 0;
+}
 int view_text_sub(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R, int64_t own_from) {
     auto& V = h->vt; cudaStream_t sm = h->s_main;
     const uint32_t n_tiles = (R + SAM_SCAN_TILE - 1) / SAM_SCAN_TILE;
@@ -740,8 +751,10 @@ int view_text_sub(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R
     SamTab t = V.tab; t.ctl = V.ctl.as<unsigned long long>();
     CK(cudaMemsetAsync(t.ctl, 0, 24, sm));
     CK(cudaEventRecord(h->ev[30], sm));
-    if (V.fmt == TEXT_JSON) BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_json_len)(soa, u0, R, own_from, h->vsel, t, len);
-    else BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_sam_len)(soa, u0, R, own_from, h->vsel, t, len);
+    ViewSel vs = h->vsel;
+    if (h->view_valid) { int rc = launch_view_valid(h, soa, u0, R, own_from, t.ctl + 2, vs); if (rc) return rc; }      // refusals share the lines' error word
+    if (V.fmt == TEXT_JSON) BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_json_len)(soa, u0, R, own_from, vs, t, len);
+    else BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_sam_len)(soa, u0, R, own_from, vs, t, len);
     BD_LAUNCH(n_tiles, 256, 0, sm, k_sam_tile_sum)(len, R, tsum);
     BD_LAUNCH(1, 1024, 0, sm, k_text_scan)(tsum, n_tiles, toff, t.ctl);
     BD_LAUNCH(n_tiles, 256, 0, sm, k_sam_scan_apply)(len, R, toff, off);
@@ -1261,7 +1274,11 @@ int consume_census(Pipe& P, const SubBatch& s, bool flagstat) {
     const int64_t own_from = (h->world > 1 && (flagstat || !P.sparse)) ? (int64_t)h->own_lo_abs_u - (int64_t)s.batch_u0 : INT64_MIN;
     CK(cudaEventRecord(h->ev[22], sm));
     if (flagstat) BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_flagstat)(s.soa, s.u0, (uint32_t)R, own_from, h->fs.as<unsigned long long>());
-    else BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_view_count)(s.soa, s.u0, (uint32_t)R, own_from, h->vsel, h->vc.as<unsigned long long>());
+    else {
+        ViewSel vs = h->vsel;
+        if (h->view_valid) { int rc = launch_view_valid(h, s.soa, s.u0, (uint32_t)R, own_from, h->vc.as<unsigned long long>() + 2, vs); if (rc) return rc; }
+        BD_LAUNCH((unsigned)((R + 255) / 256), 256, 0, sm, k_view_count)(s.soa, s.u0, (uint32_t)R, own_from, vs, h->vc.as<unsigned long long>());
+    }
     CK(cudaGetLastError()); h->st.gpu_launches++;
     CK(cudaEventRecord(h->ev[23], sm));
     P.census_timed = true;
@@ -1305,7 +1322,10 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     bool sparse_bad = false;         // a region chunk's record chain did not end at the chunk end (several ranks: decided together after the batches)
     switch (mode) {      // the consumer's tables and counters (depth's were set up above)
         case RUN_INDEX: rc = setup_index_tables(h); if (rc) return rc; break;
-        case RUN_FLAGSTAT: case RUN_VIEW_COUNT: case RUN_VIEW_TEXT: { const Census c = census_of(h, need.owes); CK(c.d.ensure(c.words * 8)); CK(cudaMemsetAsync(c.d.p, 0, c.words * 8, sm)); break; }
+        case RUN_FLAGSTAT: case RUN_VIEW_COUNT: case RUN_VIEW_TEXT: {
+            const Census c = census_of(h, need.owes); const size_t words = c.words + (mode == RUN_VIEW_COUNT ? 1 : 0);      // view -c: and -v's error word
+            CK(c.d.ensure(words * 8)); CK(cudaMemsetAsync(c.d.p, 0, words * 8, sm)); break;
+        }
         default: break;
     }
     CK(cudaEventRecord(h->ev[10], sm));
@@ -1451,7 +1471,12 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     st.ms_h2d = ms_h2d; st.ms_inflate = ms_k1; st.ms_scan = ms_k2; st.ms_coverage = ms_k3;
     h->own_lo = 0; h->own_hi = h->hdr.total_len;
     switch (mode) {
-        case RUN_FLAGSTAT: case RUN_VIEW_COUNT: rc = finish_census(h, need.owes); if (rc) return rc; st.ms_reduce = P.ms_census; break;
+        case RUN_FLAGSTAT: case RUN_VIEW_COUNT:
+            if (mode == RUN_VIEW_COUNT && h->view_valid) {      // a refusal of -v, before the ranks sum (a refusing rank joins the sum with its mark set)
+                unsigned long long e = 0; CK(cudaMemcpyAsync(&e, h->vc.as<unsigned long long>() + 2, 8, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
+                if (e) return fail(h, BDEPTH_ERR_FORMAT, "%s", sam_err_msg(e));
+            }
+            rc = finish_census(h, need.owes); if (rc) return rc; st.ms_reduce = P.ms_census; break;
         case RUN_VIEW_TEXT:
             rc = view_text_flush(h); if (rc) return rc;      // the last piece, before the ranks learn that this one is complete
             st.ms_d2h = h->vt.ms_d2h; rc = finish_census(h, need.owes); if (rc) return rc; st.ms_reduce = h->vt.ms_fmt;
@@ -1646,7 +1671,7 @@ void bdepth_close(bdepth_t* h) {
     h->seg.s.release(); h->seg.e.release(); h->seg.pmax.release(); h->seg.id.release(); h->seg.reads.release(); h->seg.minstart.release(); h->seg.bases_reads.release(); h->seg.mbases.release(); h->seg.ustart.release(); h->seg.dscr.release(); h->seg.da.release(); h->seg.dac.release(); h->seg.db.release(); h->seg.dthr.release(); h->seg.dbases.release(); h->seg.dcov.release();
     { auto& X = h->ix; X.lin.release(); X.lin_len.release(); X.lin_base.release(); X.lin_cap.release(); X.n_mapped.release(); X.n_unmapped.release(); X.carry.release(); X.ctl.release(); X.runs.release(); X.excs.release(); }
     h->m_hash.release(); h->m_flag.release(); h->m_ctl.release(); h->fprog_d.release();
-    h->vc.release(); h->vc_reg.release(); h->vc_prog.release();
+    h->vc.release(); h->vc_reg.release(); h->vc_prog.release(); h->vv.release();
     { auto& V = h->vt; V.names.release(); V.len.release(); V.off.release(); V.tiles.release(); V.ctl.release(); V.cut_r.release(); V.cut_o.release(); V.slot[0].release(); V.slot[1].release(); if (V.host) cudaFreeHost(V.host); V.host = nullptr; V.cap = 0; }
     if (h->comm) { nccl().CommDestroy(h->comm); h->comm = nullptr; }
     if (h->pinned) cudaFreeHost(h->pinned);
@@ -2214,6 +2239,8 @@ int view_setup(bdepth* h, const bdepth_view_opts* o, const bdepth_region* regs, 
     if (positional) vs.region_mode = (rg.empty() && !n_star) ? VIEW_ALL : VIEW_POSITIONAL;
     else vs.region_mode = o->regions_from == BDEPTH_VIEW_BED ? VIEW_MERGED : VIEW_ALL;
     vs.n_star = positional ? n_star : 0;
+    vs.stream_all = (vs.region_mode == VIEW_ALL || (vs.region_mode == VIEW_MERGED && !sorted)) ? 1u : 0u;      // -v: whose refusals count (kernels.cuh, view_select)
+    h->view_valid = o->valid != 0;
     if (vs.region_mode == VIEW_MERGED && rg.empty()) {
         if (!sorted) return fail(h, BDEPTH_ERR_ARG, "-L on a file that is not coordinate-sorted names no region of the file's references: the reference's BedFilter indexes an empty region list (filtering.d:128)");
         *empty = true; return 0;                                                          // getReadsOverlapping([]): an empty stream

@@ -1355,7 +1355,13 @@ __global__ void __launch_bounds__(256) k_flagstat(RecordSoA soa, const uint8_t* 
 //                    refID -1 counts n_star times ('*', unmappedReads, reader.d:370-391).
 // Reads with pos < 0 on a reference count in no region.  Records below `own_from` (offset of the block_size field, batch-relative) belong to the
 // previous rank's zone and are counted there.  Warp sum, one shared word per CTA, one 64-bit atomic per CTA.
+// -v (ValidAlignmentFilter, filtering.d:78-83) stands between -s and --num-filter (view.d:265-289: SubsampleFilter in front of the chain, then
+// the validator, FlagBitFilter, -F).  vstat holds k_view_valid's status of each record: an invalid read is dropped; a read whose tag walk the
+// reference's validator would abort on (VV status = a SAM_ERR_* code) refuses the run if the validator reaches it -- -s kept it and it is in the
+// reference's stream: every record with stream_all (no regions, -L on an unsorted file, where BedFilter comes after the validator), otherwise a
+// read with a multiplicity (getReadsOverlapping and the region readers feed the filter).  --num-filter and -F do not spare it.
 constexpr uint32_t VIEW_ALL = 0, VIEW_MERGED = 1, VIEW_POSITIONAL = 2;
+constexpr uint8_t VV_OK = 0, VV_BAD = 0xFF;      // k_view_valid's status of a record: valid, invalid, or else the SAM_ERR_* code of its refusal
 struct ViewSel {
     uint32_t flag_set, flag_unset;
     const FilterProg* fprog;                       // nullptr: no -F
@@ -1363,21 +1369,29 @@ struct ViewSel {
     uint32_t region_mode, n_star;
     uint32_t n_reg_refs;                           // references with a slice: reg_off has n_reg_refs + 1 entries
     const uint32_t* reg_off; const uint32_t* reg_s; const uint32_t* reg_e;      // regions of reference r: [reg_off[r], reg_off[r + 1]), starts and ends each sorted
+    const uint8_t* vstat;                          // -v: the sub-batch's VV_* statuses; nullptr: no -v
+    unsigned long long* verr;                      // -v: the highest SAM_ERR_* code of a refused read (atomicMax)
+    uint32_t stream_all;                           // -v: every record of the file is in the reference's stream
 };
-// The multiplicity of record r of a sub-batch under the selection (shared by k_view_count and the SAM text kernels k_sam_len).
+// The multiplicity of record r of a sub-batch under the selection (shared by k_view_count and the text kernels k_sam_len, k_json_len).
 __device__ __forceinline__ unsigned long long view_select(const RecordSoA& soa, const uint8_t* __restrict__ u, uint32_t r, int64_t own_from, const ViewSel& vs) {
     unsigned long long m = 0;
     if (soa.off[r] - 4 >= own_from) {
         const int64_t o = soa.off[r];                          // refID field
         const uint32_t flag = soa.meta[r] >> 16, ncl = soa.ncl[r], l_name = ncl & 0xFFu, n_cigar = (ncl >> 8) & 0xFFFFu;
-        bool keep = (flag & vs.flag_set) == vs.flag_set && (flag & vs.flag_unset) == 0;
+        const bool flags_ok = (flag & vs.flag_set) == vs.flag_set && (flag & vs.flag_unset) == 0;
+        bool keep = flags_ok || vs.vstat;
         if (keep && vs.subsample) {
             unsigned long long h = 14695981039346656037ull;
             for (uint32_t i = 0; i + 1 < l_name; i++) { h ^= u[o + 32 + i]; h *= 1099511628211ull; }      // read.name: l_name - 1 bytes, without the NUL
             for (int i = 0; i < 8; i++) { h ^= (vs.seed >> (8 * i)) & 0xFFu; h *= 1099511628211ull; }
             keep = (h & 0xFFFFFFFFull) < vs.threshold;
         }
+        const uint8_t st = (keep && vs.vstat) ? vs.vstat[r] : VV_OK;
+        const bool refuse = st != VV_OK && st != VV_BAD;
+        keep = keep && flags_ok && st == VV_OK;
         if (keep && vs.fprog) keep = filter_eval_cold(vs.fprog, u + o, ldu32(u + o - 4));
+        keep = keep || refuse;                                 // a refused read: is it in the stream?
         if (keep && vs.region_mode == VIEW_ALL) m = 1;
         else if (keep) {
             const int32_t ref = (int32_t)ldu32(u + o), pos = (int32_t)ldu32(u + o + 4);
@@ -1397,6 +1411,7 @@ __device__ __forceinline__ unsigned long long view_select(const RecordSoA& soa, 
                 }
             }
         }
+        if (refuse) { if (m || vs.stream_all) atomicMax(vs.verr, (unsigned long long)st); m = 0; }
     }
     return m;
 }
@@ -1663,6 +1678,40 @@ __device__ __forceinline__ int64_t sam_int(uint8_t t, const uint8_t* p) {
     }
 }
 __device__ __forceinline__ uint32_t sam_int_size(uint8_t t) { return (t == 'c' || t == 'C') ? 1u : (t == 's' || t == 'S') ? 2u : (t == 'i' || t == 'I' || t == 'f') ? 4u : 0u; }
+// One step of the tag walk (BamRead.opApply, read.d:1173-1186; readValue, tagvalue.d:468-504), taken while off + 1 < alen: the tag at aux offset
+// off has its type at off + 2, its value from off + 3 and the next tag at t.end; or the SAM_ERR_* refusal.  Every lane calls it: the warp looks
+// for the NUL of a Z / H value 32 bytes at a time.  k_view_valid's walk: sam_line's and json_line's inline walks, step for step, with their
+// checks in the same order and the same codes, without the formatting.
+struct TagAt { uint8_t ty; uint32_t val, end; };
+__device__ __forceinline__ uint32_t tag_step(const uint8_t* __restrict__ ax, uint32_t alen, uint32_t off, uint32_t lane, TagAt& t) {
+    if (off + 2 >= alen) return SAM_ERR_OVERRUN;
+    const uint8_t ty = ax[off + 2]; const uint32_t v = off + 3;
+    t.ty = ty; t.val = v;
+    if (ty == 'A') {
+        if (v + 1 > alen) return SAM_ERR_OVERRUN;
+        t.end = v + 1;
+    } else if (ty == 'c' || ty == 'C' || ty == 's' || ty == 'S' || ty == 'i' || ty == 'I' || ty == 'f') {
+        const uint32_t sz = sam_int_size(ty);
+        if (v + sz > alen) return SAM_ERR_OVERRUN;
+        t.end = v + sz;
+    } else if (ty == 'Z' || ty == 'H') {
+        uint32_t nul = alen;
+        for (uint32_t b0 = v; b0 < alen; b0 += 32) {
+            const uint32_t i = b0 + lane;
+            const unsigned z = __ballot_sync(0xFFFFFFFFu, i < alen && ax[i] == 0);
+            if (z) { nul = b0 + (uint32_t)__ffs((int)z) - 1; break; }
+        }
+        if (nul == alen) return SAM_ERR_NO_NUL;
+        t.end = nul + 1;
+    } else if (ty == 'B') {
+        if (v + 5 > alen) return SAM_ERR_OVERRUN;
+        const uint32_t n = ldu32(ax + v + 1), sz = sam_int_size(ax[v]);
+        if (!sz) return SAM_ERR_B_TYPE;
+        if ((uint64_t)n * sz > alen - (v + 5)) return SAM_ERR_OVERRUN;
+        t.end = v + 5 + n * sz;
+    } else return SAM_ERR_TAG_TYPE;
+    return 0;
+}
 
 template <bool WRITE>
 __device__ uint32_t sam_line(const uint8_t* __restrict__ p, const SamTab& t, char* __restrict__ out, uint32_t lane) {
@@ -2028,6 +2077,154 @@ __global__ void __launch_bounds__(256, 1) k_json_write(const int64_t* __restrict
     const unsigned long long base = off[r0];
     for (uint32_t r = r0 + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5); r < r1; r += nw)
         if (len[r]) json_line<true>(u + rec_off[r], t, out + (off[r] - base), lane);
+}
+
+// ---- view -v: isValid (BioD/bio/std/hts/bam/validation/alignment.d:138-562) with BooleanValidator, whose onError returns false: a read is valid
+// iff no check fails.  The checks run in _visitAlignment's order (:335-341) and the first failing one ends the read:
+//   1. name (:170-190): l_read_name - 1 bytes, none empty, none over 255 (l_read_name 0: the slice length wraps), each in [!-~] and not '@';
+//   2. position (:192-200): the raw pos in [-1, 2^29 - 2];
+//   3. qualities (:202-212): all 0xFF or all in [0, 93];
+//   4. CIGAR as written (:214-268; an empty one passes): no H but first or last of more than 2 ops; after one leading and one trailing H are
+//      dropped, no S but first or last of more than 2; with l_seq > 0, the M/I/S/=/X lengths sum to l_seq in D's int (wrapping);
+//   5. tags (:272-333,343-526), every one visited: H non-empty hex, A in [!-~], Z non-empty in [ -~]; then, for a value that passed, the
+//      predefined keys' types, quality strings, lengths and the MD grammar (vv_key); no key twice.
+// Step 5 walks the tags as opApply does (tag_step): a walk that fails there -- an unknown type, an overrun, a missing NUL -- is where the
+// reference throws or reads past the record, so the status is that SAM_ERR_* code, which view_select turns into a refusal of the run if the
+// validator reaches the read.  The name, CIGAR and quality fields lie inside block_size (K2 refuses a record otherwise).
+// A warp per record: the lanes share the name bytes, the qualities, the CIGAR ops and the bytes of each Z / H value; the tag chain is serial, the
+// MD scanner runs on lane 0, and the first VV_KEYS keys are compared pairwise from shared memory (later ones against a re-walk of the tags
+// before them: the same answer as the reference's recount).  Records below own_from are the previous rank's.
+constexpr uint32_t VV_KEYS = 256, VV_WARPS = 8;
+constexpr uint32_t VV_INT = 1, VV_STR = 2, VV_FZ = 4, VV_QUAL = 8, VV_SEQLEN = 16, VV_MD = 32;
+__device__ __forceinline__ constexpr uint32_t vv_k(char a, char b) { return (uint32_t)(uint8_t)a | ((uint32_t)(uint8_t)b << 8); }
+// PredefinedTags (:83-119): what checkTagValue (:428-526) demands of the key's value
+__device__ __forceinline__ uint32_t vv_key(uint32_t k) {
+    switch (k) {
+        case vv_k('A', 'M'): case vv_k('A', 'S'): case vv_k('C', 'M'): case vv_k('C', 'P'): case vv_k('F', 'I'): case vv_k('H', '0'): case vv_k('H', '1'):
+        case vv_k('H', '2'): case vv_k('H', 'I'): case vv_k('I', 'H'): case vv_k('M', 'Q'): case vv_k('N', 'H'): case vv_k('N', 'M'): case vv_k('O', 'P'):
+        case vv_k('P', 'Q'): case vv_k('S', 'M'): case vv_k('T', 'C'): case vv_k('U', 'Q'): return VV_INT;
+        case vv_k('B', 'C'): case vv_k('C', 'C'): case vv_k('C', 'S'): case vv_k('F', 'S'): case vv_k('L', 'B'): case vv_k('O', 'C'): case vv_k('P', 'G'):
+        case vv_k('P', 'U'): case vv_k('R', '2'): case vv_k('R', 'G'): return VV_STR;
+        case vv_k('C', 'Q'): case vv_k('O', 'Q'): case vv_k('Q', '2'): case vv_k('U', '2'): return VV_STR | VV_QUAL;
+        case vv_k('E', '2'): return VV_STR | VV_QUAL | VV_SEQLEN;
+        case vv_k('B', 'Q'): return VV_STR | VV_SEQLEN;
+        case vv_k('M', 'D'): return VV_STR | VV_MD;
+        case vv_k('F', 'Z'): return VV_FZ;
+        default: return 0;
+    }
+}
+__device__ __forceinline__ bool vv_digit(uint8_t c) { return c >= '0' && c <= '9'; }
+__device__ __forceinline__ bool vv_upper(uint8_t c) { return c >= 'A' && c <= 'Z'; }
+// the MD scanner of checkTagValue (:483-523) on a non-empty value: ^[0-9]+(([A-Z]|\^[A-Z]+)[0-9]+)*$
+__device__ __forceinline__ bool vv_md(const uint8_t* s, uint32_t n) {
+    bool valid = vv_digit(s[0]);
+    uint32_t i = 1;
+    while (i < n && vv_digit(s[i])) ++i;
+    while (i < n) {
+        if (vv_upper(s[i])) ++i;
+        else if (s[i] == '^') {
+            ++i;
+            if (i == n || !vv_upper(s[i])) { valid = false; break; }
+            while (i < n && vv_upper(s[i])) ++i;
+        } else { valid = false; break; }
+        if (i == n || !vv_digit(s[i])) { valid = false; break; }
+        while (i < n && vv_digit(s[i])) ++i;
+    }
+    return valid && i >= n;
+}
+__device__ __forceinline__ uint8_t view_valid_one(const uint8_t* __restrict__ p, uint32_t lane, uint16_t* __restrict__ keys) {
+    // p: the record's refID field
+    const uint32_t bs = ldu32(p - 4), l_name = p[8], n_cig = ldu32(p + 12) & 0xFFFFu;
+    const int32_t pos = (int32_t)ldu32(p + 4), l_seq = (int32_t)ldu32(p + 16);
+    const unsigned FULL = 0xFFFFFFFFu;
+    // 1, 2
+    if (l_name <= 1 || pos < -1 || pos > (1 << 29) - 2) return VV_BAD;
+    bool b = false;
+    for (uint32_t i = lane; i + 1 < l_name; i += 32) { const uint8_t c = p[32 + i]; b |= c < '!' || c > '~' || c == '@'; }
+    if (__ballot_sync(FULL, b)) return VV_BAD;
+    // 3
+    const uint8_t* cg = p + 32 + l_name;
+    const uint8_t* qs = cg + 4 * n_cig + ((uint32_t)l_seq + 1) / 2;
+    bool not_ff = false, over = false;
+    for (uint32_t i = lane; i < (uint32_t)l_seq; i += 32) { const uint8_t q = qs[i]; not_ff |= q != 0xFFu; over |= q > 93u; }
+    if (__ballot_sync(FULL, not_ff) && __ballot_sync(FULL, over)) return VV_BAD;
+    // 4
+    if (n_cig) {
+        const uint32_t lo = (ldu32(cg) & 15u) == 5u ? 1u : 0u, hi = n_cig - ((ldu32(cg + 4 * (n_cig - 1)) & 15u) == 5u ? 1u : 0u);      // H stripped: [lo, hi)
+        uint32_t sum = 0; bool h_in = false, s_in = false;
+        for (uint32_t i = lane; i < n_cig; i += 32) {
+            const uint32_t c = ldu32(cg + 4 * i), op = c & 15u;
+            if (cig_qcons(op)) sum += c >> 4;
+            h_in |= op == 5u && i >= 1 && i + 1 < n_cig;
+            s_in |= op == 4u && i > lo && i + 1 < hi;
+        }
+        for (int s = 16; s; s >>= 1) sum += __shfl_xor_sync(FULL, sum, s);
+        if (n_cig > 2 && __ballot_sync(FULL, h_in)) return VV_BAD;
+        if (n_cig > 2 && hi - lo > 2 && __ballot_sync(FULL, s_in)) return VV_BAD;
+        if (l_seq > 0 && sum != (uint32_t)l_seq) return VV_BAD;
+    }
+    // 5
+    const uint32_t a0 = 32u + l_name + 4u * n_cig + ((uint32_t)l_seq + 1) / 2 + (uint32_t)l_seq;
+    const uint8_t* ax = p + a0; const uint32_t alen = bs - a0;
+    bool bad = false, dup = false;
+    uint32_t k = 0;
+    for (uint32_t off = 0; off + 1 < alen; k++) {
+        TagAt tg;
+        const uint32_t err = tag_step(ax, alen, off, lane, tg);
+        if (err) return (uint8_t)err;
+        const uint32_t key = vv_k((char)ax[off], (char)ax[off + 1]);
+        const uint8_t ty = tg.ty;
+        bool tb = false;                                       // isValid (:343-405): the value's own type check
+        uint32_t n = 0; bool space = false;
+        if (ty == 'Z' || ty == 'H') {
+            n = tg.end - 1 - tg.val;
+            bool lb = false;
+            for (uint32_t i = lane; i < n; i += 32) {
+                const uint8_t c = ax[tg.val + i];
+                lb |= ty == 'H' ? !(vv_digit(c) || (c >= 'a' && c <= 'f') || (c >= 'A' && c <= 'F')) : (c < ' ' || c > '~');
+                space |= c == ' ';
+            }
+            tb = n == 0 || __ballot_sync(FULL, lb);
+            space = __ballot_sync(FULL, space) != 0;
+        } else if (ty == 'A') tb = ax[tg.val] < '!' || ax[tg.val] > '~';
+        if (!tb) {                                             // additionalChecksIfTheTagIsPredefined (:407-426)
+            const uint32_t cls = vv_key(key);
+            if (cls & VV_INT) tb = !(ty == 'c' || ty == 'C' || ty == 's' || ty == 'S' || ty == 'i' || ty == 'I');
+            else if (cls & VV_FZ) tb = !(ty == 'B' && ax[tg.val] == 'S');
+            else if (cls & VV_STR) {
+                tb = ty != 'Z' || ((cls & VV_QUAL) && space) || ((cls & VV_SEQLEN) && n != (uint32_t)l_seq);      // (a Z value here is in [ -~])
+                if (!tb && (cls & VV_MD)) tb = !__shfl_sync(FULL, lane == 0 ? (int)vv_md(ax + tg.val, n) : 0, 0);
+            }
+        }
+        bad |= tb;
+        if (!dup) {                                            // :293-322
+            if (k < VV_KEYS) {
+                bool d = false;
+                for (uint32_t j = lane; j < k; j += 32) d |= keys[j] == key;
+                dup = __ballot_sync(FULL, d) != 0;
+                __syncwarp();
+                if (lane == 0) keys[k] = (uint16_t)key;
+                __syncwarp();
+            } else {
+                for (uint32_t o2 = 0; o2 < off && !dup;) {      // the tags before this one walked again (they walked cleanly once)
+                    dup = vv_k((char)ax[o2], (char)ax[o2 + 1]) == key;
+                    TagAt t2; tag_step(ax, alen, o2, lane, t2); o2 = t2.end;
+                }
+            }
+        }
+        off = tg.end;
+    }
+    return (bad || dup) ? VV_BAD : VV_OK;
+}
+// vstat[r] = the VV_* status of record r of the sub-batch; warp per record, as k_sam_len
+__global__ void __launch_bounds__(VV_WARPS * 32) k_view_valid(RecordSoA soa, const uint8_t* __restrict__ u, uint32_t R, int64_t own_from, uint8_t* __restrict__ vstat) {
+    __shared__ uint16_t s_keys[VV_WARPS][VV_KEYS];
+    const uint32_t lane = threadIdx.x & 31, nw = gridDim.x * (blockDim.x >> 5);
+    uint16_t* keys = s_keys[threadIdx.x >> 5];
+    for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < R; r += nw) {
+        const uint8_t st = soa.off[r] - 4 >= own_from ? view_valid_one(u + soa.off[r], lane, keys) : VV_OK;
+        if (lane == 0) vstat[r] = st;
+    }
 }
 
 }  // namespace bdk

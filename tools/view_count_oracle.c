@@ -19,9 +19,12 @@
  * a Z / H value without its NUL, a reference ID outside [-1, n_ref) that is printed), the text entry point returns an error.
  * The JSON record of `view -f json` is a literal C statement of BamRead.toJson (read.d:768-830) plus '\n' with BioD's writers: writeStringJson and
  * its escape table, writeFloatJson (%g, +-1.0e+1024 for +-inf, null for NaN) and itoa (format.d:66-87,196-270); its refusals are the SAM line's.
+ * -v is a literal C statement of BioD's isValid (bio/std/hts/bam/validation/alignment.d:138-562), applied in view_main's filter chain: after
+ * SubsampleFilter, before FlagBitFilter and -F, and before BedFilter; where its tag walk throws or reads past the record, the run fails.
  * Library: view_count_oracle(), view_text_oracle(), view_json_oracle(), view_text_oracle_free(), view_count_oracle_hash(),
- * view_count_oracle_error().  With -DORACLE_MAIN also a CLI:
- *   view_count_oracle view [-c] [-f sam|json] [--num-filter=I1/I2] [-s FRAC] [--subsampling-seed=SEED] [-L BED] in.bam [region ...]
+ * view_count_oracle_error(), view_count_oracle_set_valid() (-v for the calls that follow), view_valid_oracle() (one record).  With -DORACLE_MAIN
+ * also a CLI:
+ *   view_count_oracle view [-c] [-v] [-f sam|json] [--num-filter=I1/I2] [-s FRAC] [--subsampling-seed=SEED] [-L BED] in.bam [region ...]
  * which prints the count as `sambamba view -c` does, or without -c the SAM lines or JSON records (no header), or "sambamba-view: <msg>" and exit
  * code 1 for the errors it restates. */
 #include <ctype.h>
@@ -303,12 +306,168 @@ static void emit(const Bam* b, const Rec* x, Out* o) {
     if (!o->err) (o->json ? json_line : sam_line)(b, x, o);
 }
 
-/* BamReadFilter (randomaccessmanager.d:366-462): number of records of rec[0..n) the state machine yields for the sorted, non-overlapping regions. */
-static int keep_read(const Rec* x, unsigned fs, unsigned fu, int sub, uint64_t thr, uint64_t seed) {
-    if ((x->flag & fs) != fs || (x->flag & fu)) return 0;
-    if (sub && (view_count_oracle_hash(x->name, x->l_name ? x->l_name - 1 : 0, seed) & 0xFFFFFFFFull) >= thr) return 0;
+/* ---- isValid (BioD/bio/std/hts/bam/validation/alignment.d:138-562) as BooleanValidator (:528-562) runs it: every onError returns false, so
+ * each check stops at its first failure and _visitAlignment (:335-341) stops at the first failing check.  p: the refID field, bs: block_size
+ * (the name, CIGAR, sequence and qualities lie inside it: the engine refuses the file otherwise).  Returns 0 (valid), 1 (invalid) or 2 where
+ * the tag walk throws or reads past the record (opApply, read.d:1173-1186; readValue, tagvalue.d:468-504), *why saying which. */
+typedef struct { const uint8_t* key; uint8_t t; const uint8_t* v; size_t n; } Tag;     /* n: Z / H length without the NUL, B element count */
+/* one step of opApply at offset *off of the aux bytes: 0 and the tag, or 2 and *why */
+static int tag_next(const uint8_t* ax, size_t alen, size_t* off, Tag* g, const char** why) {
+    g->key = ax + *off; *off += 2;
+    if (*off >= alen) { *why = "tag runs past the record"; return 2; }
+    const uint8_t t = ax[(*off)++]; const uint32_t sz = val_size(t);
+    g->t = t; g->v = ax + *off; g->n = 1;
+    if (t == 'A') {
+        if (*off + 1 > alen) { *why = "tag runs past the record"; return 2; }
+        *off += 1;
+    } else if (sz) {
+        if (*off + sz > alen) { *why = "tag runs past the record"; return 2; }
+        *off += sz;
+    } else if (t == 'Z' || t == 'H') {
+        const uint8_t* z = memchr(ax + *off, 0, alen - *off);
+        if (!z) { *why = "Z or H value without its NUL"; return 2; }
+        g->n = (size_t)(z - (ax + *off)); *off = (size_t)(z - ax) + 1;
+    } else if (t == 'B') {
+        if (*off + 5 > alen) { *why = "B array runs past the record"; return 2; }
+        const uint32_t n = rd32(ax + *off + 1), esz = val_size(ax[*off]); *off += 5;
+        if (!esz) { *why = "unknown B array element type"; return 2; }
+        if ((uint64_t)n * esz > alen - *off) { *why = "B array runs past the record"; return 2; }
+        g->n = n; *off += (size_t)n * esz;
+    } else { *why = "unknown tag type"; return 2; }
+    return 0;
+}
+static int is_integer(uint8_t t) { return t == 'c' || t == 'C' || t == 's' || t == 'S' || t == 'i' || t == 'I'; }
+static int key_in(const uint8_t* k, const char* list) {      /* list: keys separated by one space */
+    for (size_t i = 0; i + 1 < strlen(list); i += 3) if (k[0] == (uint8_t)list[i] && k[1] == (uint8_t)list[i + 1]) return 1;
+    return 0;
+}
+/* checkTagValue (:428-526) of a predefined key (PredefinedTags, :83-119); other keys pass (additionalChecksIfTheTagIsPredefined, :407-426) */
+static int check_tag_value(const Tag* g, int32_t l_seq) {
+    const uint8_t* k = g->key;
+    if (key_in(k, "AM AS CM CP FI H0 H1 H2 HI IH MQ NH NM OP PQ SM TC UQ")) return is_integer(g->t);      /* 1. type: int */
+    if (key_in(k, "FZ")) return g->t == 'B' && g->v[0] == 'S';                                          /*    ushort[] */
+    if (!key_in(k, "BC BQ CC CQ CS E2 FS LB MD OQ OC PG PU Q2 R2 RG U2")) return 1;
+    if (g->t != 'Z') return 0;                                                /*    string: is_string, and not 'H' */
+    const uint8_t* s = g->v; const size_t n = g->n;
+    if (key_in(k, "CQ E2 OQ Q2 U2")) {                                        /* 2. "*" or all [!-~] */
+        int all = 1; for (size_t i = 0; i < n; i++) if (!(s[i] >= '!' && s[i] <= '~')) all = 0;
+        if (!(n == 1 && s[0] == '*') && !all) return 0;
+    }
+    if (key_in(k, "BQ E2") && n != (size_t)l_seq) return 0;                  /* 3. the sequence's length */
+    if (key_in(k, "MD")) {                                                    /* 4. the scanner of :483-523 */
+        int valid = 1;
+        if (n == 0) valid = 0;
+        if (!isdigit(s[0])) valid = 0;
+        size_t i = 1;
+        while (i < n && isdigit(s[i])) ++i;
+        while (i < n) {
+            if (isupper(s[i])) ++i;
+            else if (s[i] == '^') {
+                ++i;
+                if (i == n || !isupper(s[i])) { valid = 0; break; }
+                while (i < n && isupper(s[i])) ++i;
+            } else { valid = 0; break; }
+            if (i == n || !isdigit(s[i])) { valid = 0; break; }
+            while (i < n && isdigit(s[i])) ++i;
+        }
+        if (i < n) valid = 0;
+        if (!valid) return 0;
+    }
     return 1;
 }
+/* isValid(key, value, al) (:343-405): the value's own type, then the predefined keys */
+static int tag_is_valid(const Tag* g, int32_t l_seq) {
+    if (g->t == 'H') {
+        if (g->n == 0) return 0;
+        for (size_t i = 0; i < g->n; i++) if (!isxdigit(g->v[i])) return 0;
+    } else if (g->t == 'A') {
+        if (!(g->v[0] >= '!' && g->v[0] <= '~')) return 0;
+    } else if (g->t == 'Z') {
+        if (g->n == 0) return 0;
+        for (size_t i = 0; i < g->n; i++) if (!(g->v[i] >= ' ' && g->v[i] <= '~')) return 0;
+    }
+    return check_tag_value(g, l_seq);
+}
+static int alignment_valid(const uint8_t* p, uint32_t bs, const char** why) {
+    const int32_t pos = (int32_t)rd32(p + 4), l_seq = (int32_t)rd32(p + 16);
+    const uint32_t l_name = p[8], n_cig = rd32(p + 12) & 0xFFFF;
+    /* invalidReadName (:170-190): name = the first l_read_name - 1 bytes; l_read_name 0 slices [32 .. 31], whose length wraps */
+    const size_t name_len = (size_t)l_name - 1;
+    if (name_len == 0) return 1;
+    if (name_len > 255) return 1;
+    for (size_t i = 0; i < name_len; i++) { const uint8_t c = p[32 + i]; if (c < '!' || c > '~' || c == '@') return 1; }
+    /* invalidPosition (:192-200) */
+    if (pos < -1 || pos > ((1 << 29) - 2)) return 1;
+    /* invalidQualityData (:202-212) */
+    const uint8_t* cg = p + 32 + l_name;
+    const uint8_t* qs = cg + 4 * n_cig + ((uint32_t)l_seq + 1) / 2;
+    int all_ff = 1, all_ok = 1;
+    for (int32_t i = 0; i < l_seq; i++) { if (qs[i] != 0xFF) all_ff = 0; if (qs[i] > 93) all_ok = 0; }
+    if (!all_ff && !all_ok) return 1;
+    /* invalidCigar (:214-268): op types "MIDNSHP=X????????"[op & 15] (cigar.d:110) */
+    if (n_cig) {
+        char ty[65536];
+        for (uint32_t i = 0; i < n_cig; i++) ty[i] = "MIDNSHP=X????????"[rd32(cg + 4 * i) & 15];
+        if (n_cig > 2) for (uint32_t i = 1; i + 1 < n_cig; i++) if (ty[i] == 'H') return 1;       /* internalHardClipping */
+        if (n_cig > 2) {                                                                             /* internalSoftClipping */
+            uint32_t a = 0, e = n_cig;
+            if (ty[a] == 'H') a++;
+            if (ty[e - 1] == 'H') e--;
+            if (e - a > 2) for (uint32_t i = a + 1; i + 1 < e; i++) if (ty[i] == 'S') return 1;
+        }
+        int32_t sum = 0;                                                                             /* inconsistentLength: reduce in int, wrapping */
+        for (uint32_t i = 0; i < n_cig; i++) if (strchr("MIS=X", ty[i])) sum = (int32_t)((uint32_t)sum + (rd32(cg + 4 * i) >> 4));
+        if (l_seq > 0 && l_seq != sum) return 1;
+    }
+    /* invalidTags (:272-333): every tag is visited (someTagIsBad's return leaves only that nested function) */
+    const uint32_t a0 = 32 + l_name + 4 * n_cig + ((uint32_t)l_seq + 1) / 2 + (uint32_t)l_seq;
+    const uint8_t* ax = p + a0; const size_t alen = bs - a0;
+    int all_tags_are_good = 1, all_distinct = 1;
+    uint16_t keys[256]; size_t i = 0;
+    for (size_t off = 0; off + 1 < alen;) {
+        Tag g;
+        if (tag_next(ax, alen, &off, &g, why)) return 2;
+        if (!tag_is_valid(&g, l_seq)) all_tags_are_good = 0;
+        const uint16_t k = (uint16_t)(g.key[0] | (g.key[1] << 8));
+        if (i < 256) {
+            keys[i] = k;
+            if (all_distinct) for (size_t j = 0; j < i; ++j) if (keys[i] == keys[j]) { all_distinct = 0; break; }
+            i += 1;
+        } else if (all_distinct) {                                             /* must be exactly one: count this key over all the tags */
+            int found = 0;
+            for (size_t o2 = 0; o2 + 1 < alen;) {
+                Tag g2;
+                if (tag_next(ax, alen, &o2, &g2, why)) return 2;
+                if ((uint16_t)(g2.key[0] | (g2.key[1] << 8)) == k) { if (found == 1) { all_distinct = 0; break; } ++found; }
+            }
+        }
+    }
+    return (all_tags_are_good && all_distinct) ? 0 : 1;
+}
+/* The validator alone on one record (p: its refID field): 0 valid, 1 invalid, 2 refused (view_count_oracle_error() says why). */
+int view_valid_oracle(const uint8_t* p, uint32_t bs) {
+    const char* why = NULL; g_err[0] = 0;
+    const int v = alignment_valid(p, bs, &why);
+    if (v == 2) snprintf(g_err, sizeof g_err, "%s", why);
+    return v;
+}
+static int g_valid;
+/* -v for the calls that follow (the existing entry points keep their signatures) */
+void view_count_oracle_set_valid(int on) { g_valid = on != 0; }
+
+/* The filter chain of view_main (view.d:265-289): SubsampleFilter in front, then NullFilter, ValidAlignmentFilter (-v), FlagBitFilter; -F comes
+ * after them (the tests apply it to the file).  A record the validator would abort on stops the run (o's error). */
+static int keep_read(const Rec* x, unsigned fs, unsigned fu, int sub, uint64_t thr, uint64_t seed, Out* o) {
+    if (sub && (view_count_oracle_hash(x->name, x->l_name ? x->l_name - 1 : 0, seed) & 0xFFFFFFFFull) >= thr) return 0;
+    if (g_valid) {
+        const char* why = NULL; const int v = alignment_valid(x->p, x->bs, &why);
+        if (v == 2) { sam_fail(o, why); return 0; }
+        if (v) return 0;
+    }
+    if ((x->flag & fs) != fs || (x->flag & fu)) return 0;
+    return 1;
+}
+/* BamReadFilter (randomaccessmanager.d:366-462): number of records of rec[0..n) the state machine yields for the sorted, non-overlapping regions. */
 static void read_filter_walk(const Bam* b, const Reg* regs, size_t nreg, size_t i0, unsigned fs, unsigned fu, int sub, uint64_t thr, uint64_t seed, Out* out) {
     size_t ri = 0; const uint32_t ref_id = regs[0].ref;
     for (size_t i = i0; i < b->nr && ri < nreg;) {
@@ -321,7 +480,7 @@ static void read_filter_walk(const Bam* b, const Reg* regs, size_t nreg, size_t 
         if ((uint32_t)x->pos > regs[ri].start) yield = 1;
         else if ((int64_t)(int32_t)x->pos + x->bc <= (int64_t)regs[ri].start) yield = 0;
         else yield = 1;
-        if (yield && keep_read(x, fs, fu, sub, thr, seed)) emit(b, x, out);
+        if (yield && keep_read(x, fs, fu, sub, thr, seed, out)) emit(b, x, out);
         i++;
     }
 }
@@ -340,7 +499,7 @@ static int view_stream(const Bam* b, unsigned flag_set, unsigned flag_unset, int
                        int mode, const uint32_t* regs, size_t nreg, unsigned n_star, Out* out) {
     int rc = 0;
     if (mode == 0) {
-        for (size_t i = 0; i < b->nr; i++) if (keep_read(&b->r[i], flag_set, flag_unset, subsample, threshold, seed)) emit(b, &b->r[i], out);
+        for (size_t i = 0; i < b->nr; i++) if (keep_read(&b->r[i], flag_set, flag_unset, subsample, threshold, seed, out)) emit(b, &b->r[i], out);
     } else if (mode == 1) {
         Reg* r = malloc((nreg + 1) * sizeof(Reg)); size_t m = 0;
         for (size_t i = 0; i < nreg; i++) if (regs[3 * i + 1] < regs[3 * i + 2]) { r[m].ref = regs[3 * i]; r[m].start = regs[3 * i + 1]; r[m].end = regs[3 * i + 2]; m++; }
@@ -356,7 +515,8 @@ static int view_stream(const Bam* b, unsigned flag_set, unsigned flag_unset, int
             const uint32_t ntrees = r[m - 1].ref + 1;
             for (size_t i = 0; i < b->nr; i++) {
                 const Rec* x = &b->r[i];
-                if (x->ref < 0 || (uint32_t)x->ref >= ntrees || !keep_read(x, flag_set, flag_unset, subsample, threshold, seed)) continue;
+                if (!keep_read(x, flag_set, flag_unset, subsample, threshold, seed, out)) continue;      /* the chain, then BedFilter */
+                if (x->ref < 0 || (uint32_t)x->ref >= ntrees) continue;
                 const uint32_t s = (uint32_t)x->pos, t = (uint32_t)((int32_t)x->pos + (int32_t)x->bc);
                 for (size_t j = 0; j < m; j++) if (r[j].ref == (uint32_t)x->ref && r[j].end > s && r[j].start < t) { emit(b, x, out); break; }
             }
@@ -373,11 +533,11 @@ static int view_stream(const Bam* b, unsigned flag_set, unsigned flag_unset, int
             if (one.ref != 0xFFFFFFFFu) { read_filter_walk(b, &one, 1, 0, flag_set, flag_unset, subsample, threshold, seed, out); continue; }
             /* '*' in its place: unmappedReads, the first refID -1 record, then everything to EOF */
             size_t k = 0; while (k < b->nr && b->r[k].ref != -1) k++;
-            for (; k < b->nr; k++) if (keep_read(&b->r[k], flag_set, flag_unset, subsample, threshold, seed)) emit(b, &b->r[k], out);
+            for (; k < b->nr; k++) if (keep_read(&b->r[k], flag_set, flag_unset, subsample, threshold, seed, out)) emit(b, &b->r[k], out);
         }
         for (unsigned k = 0; k < n_star && !rc; k++) {     /* unmappedReads: the first refID -1 record, then everything to EOF */
             size_t i = 0; while (i < b->nr && b->r[i].ref != -1) i++;
-            for (; i < b->nr; i++) if (keep_read(&b->r[i], flag_set, flag_unset, subsample, threshold, seed)) emit(b, &b->r[i], out);
+            for (; i < b->nr; i++) if (keep_read(&b->r[i], flag_set, flag_unset, subsample, threshold, seed, out)) emit(b, &b->r[i], out);
         }
     }
     if (!rc && out->err) rc = -1;
@@ -454,6 +614,7 @@ int main(int argc, char** argv) {
     for (int i = 2; i < argc; i++) {
         const char* a = argv[i];
         if (!strcmp(a, "-c")) count = 1;
+        else if (!strcmp(a, "-v")) g_valid = 1;
         else if (!strncmp(a, "--num-filter=", 13)) {
             char buf[256]; snprintf(buf, sizeof buf, "%s", a + 13); char* sl = strchr(buf, '/');
             if (sl) *sl = 0;
