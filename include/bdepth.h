@@ -27,6 +27,8 @@
  *     (BamRead.toSam per read)           utils/view/alignmentrangeprocessor.d:97-106
  *   JsonSerializer over view_main's     sambamba/view.d:265-379,        bdepth_run_view_json (`sambamba view -f json`)
  *     reads (BamRead.toJson per read)    utils/view/alignmentrangeprocessor.d:149-158
+ *   BamSerializer over view_main's      sambamba/view.d:380-386,        bdepth_run_view_bam (`sambamba view -f bam`)
+ *     reads (BamWriter, bgzfCompress)    utils/view/alignmentrangeprocessor.d:108-147
  *   ValidAlignmentFilter (isValid)       utils/common/filtering.d:78-83, bdepth_view_opts.valid (`view -v`, for the three
  *                                        bio/std/hts/bam/validation/alignment.d   view entry points above)
  *
@@ -321,6 +323,23 @@ int bdepth_run_view_text(bdepth_t* h, const bdepth_view_opts* opts, bdepth_text_
  * BDEPTH_ERR_FORMAT refusals and messages, the several-rank join and its refusals.
  * Timings: ms_inflate, ms_scan, ms_reduce (formatting kernels), ms_d2h (text copies), summed over the runs of a positional query. */
 int bdepth_run_view_json(bdepth_t* h, const bdepth_view_opts* opts, bdepth_text_cb cb, void* user);
+/* `sambamba view -f bam` without the .bai: exactly the bytes BamSerializer (utils/view/alignmentrangeprocessor.d:108-147) writes through BamWriter
+ * (BioD/bio/std/hts/bam/writer.d) and BgzfOutputStream (bio/core/bgzf/outputstream.d), given the header text header_text[0, header_len) (view
+ * passes SamHeader re-serialized after addPG) and the compression level (-1 or 0-9; otherwise BDEPTH_ERR_ARG "Compression level must be a number
+ * in interval [-1, 9]").  The stream is BAM\1, l_text, the text, n_ref and the handle's reference list, one member boundary, then each selected
+ * read as block_size and its bytes, with bin recomputed as reg2bin(pos, pos + basesCovered) and the last byte of the read name zeroed
+ * (read.d:616; with l_read_name 0 that is the top byte of tlen).  Members are cut as BamWriter cuts them: a read that does not fit behind the
+ * bytes written since the last flush (0xFF00 at most) flushes first, and a member also closes whenever it reaches 0xFF00 bytes, so a larger
+ * read spans members.  Each member is bgzfCompress's frame (MTIME 0, XFL 0, OS 255, BC subfield, BSIZE - 1, raw DEFLATE, CRC32, ISIZE); the
+ * stream ends with the 28-byte BGZF EOF member.  Level 0 is one stored block per member, the reference's file byte for byte.  Levels -1 and 1-9
+ * all run the GPU compressor (bgzf_deflate.cuh): the member boundaries, headers, CRC32, ISIZE and inflated bytes are the reference's, the
+ * DEFLATE bytes are not zlib's (DESIGN.md section 8).  cb gets runs of whole members, in order, from pinned memory reused once it returns; the
+ * last call is the EOF member; non-zero stops the run with BDEPTH_ERR_CALLBACK.  The selection, options, order and refusals are
+ * bdepth_run_view_text's, plus BDEPTH_ERR_FORMAT "Read reference ID is out of range" for a selected read whose refID is neither -1 nor below
+ * n_ref as unsigned (writeRecord; the mate's is not checked).  Positional regions form one stream with one header and one member cut.  Several
+ * ranks and bdepth_add_input handles are BDEPTH_ERR_ARG.  Timings: ms_inflate, ms_scan, ms_reduce (gather, member cut and compression), ms_d2h
+ * (member copies), summed over the runs of a positional query. */
+int bdepth_run_view_bam(bdepth_t* h, const bdepth_view_opts* opts, const char* header_text, size_t header_len, int level, bdepth_text_cb cb, void* user);
 /* Scan records on the GPU; copy out up to cap rows of the columnar SoA (any pointer may be NULL). */
 int64_t bdepth_scan_to_host(bdepth_t* h, uint64_t cap, int32_t* ref_id, int32_t* pos, uint32_t* span, uint16_t* flag, uint8_t* mapq, uint16_t* n_cigar, uint64_t* rec_off);
 

@@ -146,6 +146,7 @@ def load_library():
     L.bdepth_run_view_count.argtypes = [vp, C.POINTER(ViewOpts), C.POINTER(C.c_uint64)]
     L.bdepth_run_view_text.argtypes = [vp, C.POINTER(ViewOpts), TEXT_CB, vp]
     L.bdepth_run_view_json.argtypes = [vp, C.POINTER(ViewOpts), TEXT_CB, vp]
+    L.bdepth_run_view_bam.argtypes = [vp, C.POINTER(ViewOpts), C.c_char_p, C.c_size_t, C.c_int, TEXT_CB, vp]
     _lib = L
     return L
 
@@ -157,6 +158,7 @@ EXPORTED_SYMBOLS = [
     "bdepth_set_shard", "bdepth_nccl_unique_id", "bdepth_plan_shards", "bdepth_plan_region_chunks", "bdepth_set_tuning", "bdepth_stage", "bdepth_run_resident", "bdepth_run_base", "bdepth_run_base_text",
     "bdepth_run_windows", "bdepth_run_regions", "bdepth_get_stats", "bdepth_ref_has_reads", "bdepth_inflate_to_host", "bdepth_scan_to_host", "bdepth_build_index",
     "bdepth_run_flagstat", "bdepth_run_view_count", "bdepth_run_view_text", "bdepth_run_view_json",
+    "bdepth_run_view_bam",
 ]
 
 
@@ -461,6 +463,14 @@ class BDepth:
         """`sambamba view -f json`: the JSON records of the selected reads, one per line.  Keywords, order, return value and sink as in
         run_view_text."""
         return self._run_lines(self.L.bdepth_run_view_json, sink, self._view_opts(num_filter, query, subsample, seed, bed, regions, valid=valid))
+
+    def run_view_bam(self, header_text, level=-1, num_filter=(0, 0), query=None, subsample=None, seed=0, bed=None, regions=None, sink=None, valid=False):
+        """`sambamba view -f bam`: the BAM file of the selected reads, with header_text (str or bytes) as its header text, at compression level
+        -1 or 0-9 (bdepth_run_view_bam).  Keywords, order and sink as in run_view_text; the sink gets runs of whole BGZF members, the last one
+        the EOF member.  Returns the file's bytes, or with a sink their number."""
+        ht = header_text.encode() if isinstance(header_text, str) else bytes(header_text)
+        return self._run_lines(lambda h, o, cb, u: self.L.bdepth_run_view_bam(h, o, ht, len(ht), level, cb, u), sink,
+                               self._view_opts(num_filter, query, subsample, seed, bed, regions, valid=valid))
 
     def scan(self, cap):
         cols = dict(ref_id=np.zeros(cap, np.int32), pos=np.zeros(cap, np.int32), span=np.zeros(cap, np.uint32),

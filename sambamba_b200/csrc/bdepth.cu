@@ -94,8 +94,8 @@ constexpr size_t EMIT_CHUNK = 4ull << 20;     // positions per D2H chunk
 constexpr uint32_t SHARD_EXTRA_BLOCKS = 8;
 constexpr uint32_t MATE_ZONE_BLOCKS = 64;       // -m on several ranks: blocks read behind the shard so that pairs cut by the boundary are seen whole
 
-enum RunMode { RUN_FULL = 0, RUN_INFLATE_ONLY = 1, RUN_SCAN_ONLY = 2, RUN_INDEX = 3, RUN_FLAGSTAT = 4, RUN_VIEW_COUNT = 5, RUN_VIEW_TEXT = 6 };
-enum TextFormat { TEXT_SAM, TEXT_JSON };      // the lines of RUN_VIEW_TEXT: BamRead.toSam or BamRead.toJson
+enum RunMode { RUN_FULL = 0, RUN_INFLATE_ONLY = 1, RUN_SCAN_ONLY = 2, RUN_INDEX = 3, RUN_FLAGSTAT = 4, RUN_VIEW_COUNT = 5, RUN_VIEW_TEXT = 6, RUN_VIEW_BAM = 7 };
+enum TextFormat { TEXT_SAM, TEXT_JSON, TEXT_BAM };      // the lines of RUN_VIEW_TEXT: BamRead.toSam or BamRead.toJson; or BGZF members (RUN_VIEW_BAM)
 // Several ranks with NCCL: the collective of the current run that a rank owes its peers next.  A rank that stops with an error joins it with
 // a "failed" mark (abort_collectives), so that the others stop too instead of waiting for it.
 // BOUNDARY_TABLE: depth's all-gather in exchange_boundaries; SPARSE_DECISION: a sparse region query's all-reduce that tells whether every rank's
@@ -112,6 +112,7 @@ constexpr ModeNeeds MODE_NEEDS[] = {      // indexed by RunMode
     {false, false, true, false, true, Owed::NOTHING}, /* RUN_SCAN_ONLY */           {true, false, true, false, true, Owed::NOTHING}, /* RUN_INDEX */
     {true, false, false, false, true, Owed::FLAGSTAT_SUM}, /* RUN_FLAGSTAT */       {true, true, false, false, true, Owed::VIEW_SUM}, /* RUN_VIEW_COUNT */
     {true, true, false, false, true, Owed::VIEW_SUM}, /* RUN_VIEW_TEXT */
+    {true, true, false, false, true, Owed::VIEW_SUM}, /* RUN_VIEW_BAM */
 };
 constexpr const char* MSG_PEER_STOPPED = "another rank of the run stopped with an error (its own message says why): no result";
 constexpr const char* MSG_CHUNK_MISMATCH = "the index does not describe this file (a region chunk does not end at a record)";
@@ -253,6 +254,13 @@ struct bdepth {
         SamTab tab{};                                  // the reference names on the device, as the format prints them (ctl is set per sub-batch)
         TextFormat fmt = TEXT_SAM;                     // which line view_text_sub formats: SAM (bdepth_run_view_text) or JSON (bdepth_run_view_json)
     } vt;
+    // ---- view -f bam (bdepth_run_view_bam): the stage of a sub-batch (the open member's bytes carried in front of the gathered reads), the member
+    // cut's tables, the members' compressed bytes (BGZF_SLOT apart), and the cut state that passes from one sub-batch and run to the next:
+    // P bytes of the open member in `carry`, cur = BamWriter._current_size.  Delivery goes through vt's slots.
+    struct ViewBam {
+        DevBuf stage, carry, len, off, tiles, ctiles, ctl, nx, mark, cnt, base, m_off, m_len, comp, clen, coff, tok;
+        uint32_t P = 0; unsigned long long cur = 0; int level = -1;
+    } vb;
     // ---- several BAM files (bdepth_add_input; MultiBamReader, multireader.d:218-268): the additional files are whole handles that
     // only hold their input (file, BGZF members, header, index, shard / sparse plan); a run swaps them into this handle one after
     // the other and accumulates into the same counters -- per-position counters and per-segment sums are additive over reads,
@@ -802,6 +810,82 @@ int view_text_sub(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R
     return 0;
 }
 
+// ---- view -f bam (RUN_VIEW_BAM).  Per sub-batch: k_bam_len sizes the selected reads, the SAM scan gives their offsets, k_bam_write gathers
+// them behind the carried bytes of the open member, the member cut (k_bam_next .. k_bam_members) lists the members that close, k_bgzf_deflate
+// compresses them, and they go out through the text slots in pieces of whole members (k_bgzf_pack).  The open member's bytes move to `carry`.
+int bam_scan(bdepth* h, const uint32_t* len, uint32_t n, DevBuf& tiles, unsigned long long* off, unsigned long long* total) {
+    const uint32_t n_tiles = (n + SAM_SCAN_TILE - 1) / SAM_SCAN_TILE;
+    const size_t toff_at = ((size_t)n_tiles * 4 + 7) / 8 * 8;
+    CK(tiles.ensure(toff_at + (size_t)n_tiles * 8 + 8));
+    uint32_t* tsum = tiles.as<uint32_t>(); unsigned long long* toff = (unsigned long long*)(tiles.as<uint8_t>() + toff_at);
+    BD_LAUNCH(n_tiles, 256, 0, h->s_main, k_sam_tile_sum)(len, n, tsum);
+    BD_LAUNCH(1, 1024, 0, h->s_main, k_text_scan)(tsum, n_tiles, toff, total);
+    BD_LAUNCH(n_tiles, 256, 0, h->s_main, k_sam_scan_apply)(len, n, toff, off);
+    CK(cudaGetLastError()); h->st.gpu_launches += 3;
+    return 0;
+}
+// Compress the nm members listed in vb.m_off / vb.m_len (offsets into stage) and hand them to the callback, in order.  ev[30] was recorded
+// by the caller where its GPU work began: that span is counted in the formatting time.
+int bam_emit(bdepth* h, const uint8_t* stage, uint32_t nm) {
+    auto& B = h->vb; auto& V = h->vt; cudaStream_t sm = h->s_main;
+    CK(B.comp.ensure((size_t)nm * BGZF_SLOT)); CK(B.clen.ensure((size_t)nm * 4)); CK(B.coff.ensure((size_t)nm * 8 + 8)); CK(B.ctl.ensure(128));
+    const uint32_t grid = std::min<uint32_t>(nm, (uint32_t)std::max(1, h->n_sm));
+    CK(B.tok.ensure((size_t)grid * DF_THREADS * 256 * 4));
+    CK(cudaFuncSetAttribute(k_bgzf_deflate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DF_SMEM));
+    BD_LAUNCH(grid, DF_THREADS, DF_SMEM, sm, k_bgzf_deflate)(stage, B.m_off.as<unsigned long long>(), B.m_len.as<uint32_t>(), nm, B.level, B.comp.as<uint8_t>(), B.clen.as<uint32_t>(), B.tok.as<uint32_t>());
+    CK(cudaGetLastError()); h->st.gpu_launches++;
+    unsigned long long* tot_d = B.ctl.as<unsigned long long>() + 8;
+    unsigned long long* coff = B.coff.as<unsigned long long>();
+    int rc = bam_scan(h, B.clen.as<uint32_t>(), nm, B.ctiles, coff, tot_d); if (rc) return rc;
+    CK(cudaEventRecord(h->ev[31], sm));
+    unsigned long long total = 0; CK(cudaMemcpyAsync(&total, tot_d, 8, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
+    { float tm = 0; CK(cudaEventElapsedTime(&tm, h->ev[30], h->ev[31])); V.ms_fmt += tm; }
+    const uint64_t piece = std::max<uint64_t>(1, std::min<uint64_t>(VIEW_TEXT_PIECE, h->batch_u));
+    if (piece + BGZF_SLOT > V.cap) {      // a slot holds a piece and one more member: grow both, after handing out what is pending in them
+        rc = view_text_flush(h); if (rc) return rc;
+        if (V.host) { cudaFreeHost(V.host); V.host = nullptr; }
+        V.cap = 0;
+        const size_t need = piece + BGZF_SLOT;
+        CK(cudaMallocHost((void**)&V.host, 2 * need)); CK(V.slot[0].ensure(need)); CK(V.slot[1].ensure(need));
+        V.cap = need;
+    }
+    const uint32_t n_cuts = (uint32_t)((total + piece - 1) / piece) + 1;
+    CK(V.cut_r.ensure((size_t)n_cuts * 4)); CK(V.cut_o.ensure((size_t)n_cuts * 8));
+    BD_LAUNCH((n_cuts + 255) / 256, 256, 0, sm, k_sam_cut)(coff, nm, total, piece, n_cuts, V.cut_r.as<uint32_t>(), V.cut_o.as<unsigned long long>());
+    CK(cudaGetLastError()); h->st.gpu_launches++;
+    std::vector<uint32_t> cr(n_cuts); std::vector<unsigned long long> co(n_cuts);
+    CK(cudaMemcpyAsync(cr.data(), V.cut_r.p, (size_t)n_cuts * 4, cudaMemcpyDeviceToHost, sm)); CK(cudaMemcpyAsync(co.data(), V.cut_o.p, (size_t)n_cuts * 8, cudaMemcpyDeviceToHost, sm));
+    CK(cudaStreamSynchronize(sm));
+    for (uint32_t j = 0; j + 1 < n_cuts; j++) {
+        const uint32_t m0 = cr[j], m1 = j + 2 == n_cuts ? nm : cr[j + 1];
+        const uint64_t bytes = (j + 2 == n_cuts ? total : co[j + 1]) - co[j];
+        if (!bytes) continue;
+        const int s = V.next;
+        rc = view_text_deliver(h, s); if (rc) return rc;
+        CK(cudaEventRecord(h->ev[28 + s], sm));
+        BD_LAUNCH(std::min<uint32_t>(m1 - m0, 4096), 256, 0, sm, k_bgzf_pack)(B.comp.as<uint8_t>(), B.clen.as<uint32_t>(), coff, m0, m1, V.slot[s].as<uint8_t>());
+        CK(cudaGetLastError()); h->st.gpu_launches++;
+        CK(cudaEventRecord(h->ev[24 + s], sm));
+        CK(cudaStreamWaitEvent(h->s_d2h, h->ev[24 + s], 0));
+        CK(cudaMemcpyAsync(V.host + (size_t)s * V.cap, V.slot[s].p, bytes, cudaMemcpyDeviceToHost, h->s_d2h));
+        CK(cudaEventRecord(h->ev[26 + s], h->s_d2h));
+        V.pend[s] = true; V.pend_len[s] = bytes; V.next = s ^ 1;
+        rc = view_text_deliver(h, s ^ 1); if (rc) return rc;
+    }
+    return 0;
+}
+// Members of BGZF_BLOCK bytes over n bytes at stage (the last one shorter): the header and reference list, and the last open member.
+int bam_emit_run(bdepth* h, const uint8_t* stage, uint64_t n) {
+    auto& B = h->vb;
+    const uint32_t nm = (uint32_t)((n + BGZF_BLOCK - 1) / BGZF_BLOCK);
+    if (!nm) return 0;
+    std::vector<unsigned long long> mo(nm); std::vector<uint32_t> ml(nm);
+    for (uint32_t k = 0; k < nm; k++) { mo[k] = (unsigned long long)k * BGZF_BLOCK; ml[k] = (uint32_t)std::min<uint64_t>(BGZF_BLOCK, n - mo[k]); }
+    CK(B.m_off.ensure((size_t)nm * 8)); CK(B.m_len.ensure((size_t)nm * 4));
+    CK(cudaMemcpy(B.m_off.p, mo.data(), (size_t)nm * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(B.m_len.p, ml.data(), (size_t)nm * 4, cudaMemcpyHostToDevice));
+    CK(cudaEventRecord(h->ev[30], h->s_main));
+    return bam_emit(h, stage, nm);
+}
 // ---- the record pipeline: one front end shared by every run mode (H2D, K1 inflate, the K2 record-chain walk with its host verification,
 // K2 decode) hands each sub-batch of decoded records to the consumer of the run mode (the switch in run_pipeline_body).
 struct SubBatch {      // a sub-batch: R records decoded into soa from the inflated bytes at u0 (absolute offset batch_u0, ub bytes); ss: K2's statistics;
@@ -1289,6 +1373,58 @@ int consume_view_text(Pipe& P, const SubBatch& s) {
     bdepth* h = P.h; CK(cudaEventRecord(h->ev[4], h->s_main));
     return s.R ? view_text_sub(h, s.soa, s.u0, (uint32_t)s.R, (h->world > 1 && !P.sparse) ? (int64_t)h->own_lo_abs_u - (int64_t)s.batch_u0 : INT64_MIN) : 0;
 }
+int consume_view_bam(Pipe& P, const SubBatch& s) {
+    bdepth* h = P.h; cudaStream_t sm = h->s_main; auto& B = h->vb;
+    CK(cudaEventRecord(h->ev[4], sm));
+    if (!s.R) return 0;
+    const uint32_t R = (uint32_t)s.R;
+    CK(B.len.ensure((size_t)R * 4)); CK(B.off.ensure((size_t)R * 8 + 8)); CK(B.ctl.ensure(128));
+    unsigned long long* ctl = B.ctl.as<unsigned long long>();      // [0] bytes gathered, [2] error, [3] P', [4] cur', [5] members, [7] s0
+    uint32_t* len = B.len.as<uint32_t>(); unsigned long long* off = B.off.as<unsigned long long>();
+    CK(cudaMemsetAsync(ctl, 0, 64, sm));
+    CK(cudaEventRecord(h->ev[30], sm));
+    ViewSel vs = h->vsel;
+    if (h->view_valid) { int rc = launch_view_valid(h, s.soa, s.u0, R, INT64_MIN, ctl + 2, vs); if (rc) return rc; }
+    BD_LAUNCH((R + 255) / 256, 256, 0, sm, k_bam_len)(s.soa, s.u0, R, INT64_MIN, vs, (uint32_t)h->hdr.ref_len.size(), ctl + 2, len);
+    CK(cudaGetLastError()); h->st.gpu_launches++;
+    int rc = bam_scan(h, len, R, B.tiles, off, ctl); if (rc) return rc;
+    unsigned long long c[3]; CK(cudaMemcpyAsync(c, ctl, 24, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
+    if (c[2]) return fail(h, BDEPTH_ERR_FORMAT, "%s", c[2] == BAM_ERR_REF ? "Read reference ID is out of range" : sam_err_msg(c[2]));
+    const unsigned long long total = c[0];
+    if (!total) { CK(cudaEventRecord(h->ev[31], sm)); CK(cudaStreamSynchronize(sm)); float tm = 0; CK(cudaEventElapsedTime(&tm, h->ev[30], h->ev[31])); h->vt.ms_fmt += tm; return 0; }
+    h->vt.issued += total;      // (records that joined the open member are output: a restart of the run would repeat them)
+    CK(B.stage.ensure(B.P + total + 16));
+    uint8_t* stage = B.stage.as<uint8_t>();
+    if (B.P) CK(cudaMemcpyAsync(stage, B.carry.p, B.P, cudaMemcpyDeviceToDevice, sm));
+    BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_bam_write)(s.soa, s.u0, R, len, off, stage + B.P);
+    // the member cut: the chain of group starts by pointer doubling over K levels (2^K covers every group of the sub-batch: two groups in a
+    // row hold more than BGZF_BLOCK bytes)
+    const unsigned long long groups = std::min<unsigned long long>(R, 2 * (B.P + total) / BGZF_BLOCK + 3);
+    uint32_t K = 1; while ((1ull << K) < groups + 1) K++;
+    CK(B.nx.ensure((size_t)(R + 1) * 4 * K)); CK(B.mark.ensure((size_t)R + 1)); CK(B.cnt.ensure((size_t)(R + 1) * 4)); CK(B.base.ensure((size_t)(R + 1) * 8 + 8));
+    uint32_t* J = B.nx.as<uint32_t>(); uint8_t* mark = B.mark.as<uint8_t>(); uint32_t* s0 = (uint32_t*)(ctl + 7);
+    const unsigned g = (unsigned)std::min<uint64_t>((R + 256) / 256, 4096);
+    CK(cudaMemsetAsync(mark, 0, (size_t)R + 1, sm));
+    BD_LAUNCH(g, 256, 0, sm, k_bam_next)(off, R, total, J);
+    for (uint32_t k = 1; k < K; k++) BD_LAUNCH(g, 256, 0, sm, k_bam_jump)(J + (size_t)(k - 1) * (R + 1), J + (size_t)k * (R + 1), R);
+    BD_LAUNCH(1, 1, 0, sm, k_bam_start)(off, R, total, B.cur, mark, s0);
+    for (uint32_t k = K; k-- > 0;) BD_LAUNCH(g, 256, 0, sm, k_bam_mark)(J + (size_t)k * (R + 1), mark, R);
+    BD_LAUNCH(g, 256, 0, sm, k_bam_members<false>)(off, R, total, J, mark, s0, B.P, B.cur, B.cnt.as<uint32_t>(), nullptr, nullptr, nullptr, nullptr);
+    CK(cudaGetLastError()); h->st.gpu_launches += 2 * K + 3;
+    rc = bam_scan(h, B.cnt.as<uint32_t>(), R + 1, B.tiles, B.base.as<unsigned long long>(), ctl + 5); if (rc) return rc;
+    const unsigned long long max_m = 3 * (B.P + total) / BGZF_BLOCK + 4;
+    CK(B.m_off.ensure(max_m * 8)); CK(B.m_len.ensure(max_m * 4));
+    BD_LAUNCH(g, 256, 0, sm, k_bam_members<true>)(off, R, total, J, mark, s0, B.P, B.cur, B.cnt.as<uint32_t>(), B.base.as<unsigned long long>(),
+                                                  B.m_off.as<unsigned long long>(), B.m_len.as<uint32_t>(), ctl + 3);
+    CK(cudaGetLastError()); h->st.gpu_launches++;
+    CK(cudaMemcpyAsync(c, ctl + 3, 24, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
+    const uint32_t P2 = (uint32_t)c[0]; const unsigned long long cur2 = c[1]; const uint32_t nm = (uint32_t)c[2];
+    if (nm) { rc = bam_emit(h, stage, nm); if (rc) return rc; }
+    else { CK(cudaEventRecord(h->ev[31], sm)); CK(cudaStreamSynchronize(sm)); float tm = 0; CK(cudaEventElapsedTime(&tm, h->ev[30], h->ev[31])); h->vt.ms_fmt += tm; }
+    if (P2) { CK(B.carry.ensure(BGZF_BLOCK)); CK(cudaMemcpyAsync(B.carry.p, stage + B.P + total - P2, P2, cudaMemcpyDeviceToDevice, sm)); }
+    B.P = P2; B.cur = cur2;
+    return 0;
+}
 int refuse_index_after_text(bdepth* h) { return fail(h, BDEPTH_ERR_FORMAT, "%s, found after SAM lines were delivered", MSG_CHUNK_MISMATCH); }
 
 // The pipeline: leaves the per-position counters of the whole shard in h->counts (RUN_FULL).
@@ -1322,7 +1458,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     bool sparse_bad = false;         // a region chunk's record chain did not end at the chunk end (several ranks: decided together after the batches)
     switch (mode) {      // the consumer's tables and counters (depth's were set up above)
         case RUN_INDEX: rc = setup_index_tables(h); if (rc) return rc; break;
-        case RUN_FLAGSTAT: case RUN_VIEW_COUNT: case RUN_VIEW_TEXT: {
+        case RUN_FLAGSTAT: case RUN_VIEW_COUNT: case RUN_VIEW_TEXT: case RUN_VIEW_BAM: {
             const Census c = census_of(h, need.owes); const size_t words = c.words + (mode == RUN_VIEW_COUNT ? 1 : 0);      // view -c: and -v's error word
             CK(c.d.ensure(words * 8)); CK(cudaMemsetAsync(c.d.p, 0, words * 8, sm)); break;
         }
@@ -1434,6 +1570,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             case RUN_FLAGSTAT: rc = consume_census(P, s, true); break;
             case RUN_VIEW_COUNT: rc = consume_census(P, s, false); break;
             case RUN_VIEW_TEXT: rc = consume_view_text(P, s); break;
+            case RUN_VIEW_BAM: rc = consume_view_bam(P, s); break;
             case RUN_INFLATE_ONLY: break;
         }
         if (rc) return rc;
@@ -1465,7 +1602,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             if (flag >= SPARSE_PEER_FAILED) { h->coll_pending = Owed::NOTHING; return fail(h, BDEPTH_ERR_NCCL, "%s", MSG_PEER_STOPPED); }
             sparse_bad = flag != 0;
         } else if (sparse_bad) return fail(h, BDEPTH_ERR_FORMAT, "%s; several ranks without a NCCL id cannot fall back together", MSG_CHUNK_MISMATCH);
-        if (sparse_bad && mode == RUN_VIEW_TEXT) return refuse_index_after_text(h);      // (the view sum is still owed: abort_collectives joins it)
+        if (sparse_bad && (mode == RUN_VIEW_TEXT || mode == RUN_VIEW_BAM)) return refuse_index_after_text(h);      // (the view sum is still owed: abort_collectives joins it)
         if (sparse_bad) { h->sparse_ok = false; CK(cudaDeviceSynchronize()); return RC_RESTART; }
     }
     st.ms_h2d = ms_h2d; st.ms_inflate = ms_k1; st.ms_scan = ms_k2; st.ms_coverage = ms_k3;
@@ -1477,7 +1614,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
                 if (e) return fail(h, BDEPTH_ERR_FORMAT, "%s", sam_err_msg(e));
             }
             rc = finish_census(h, need.owes); if (rc) return rc; st.ms_reduce = P.ms_census; break;
-        case RUN_VIEW_TEXT:
+        case RUN_VIEW_TEXT: case RUN_VIEW_BAM:
             rc = view_text_flush(h); if (rc) return rc;      // the last piece, before the ranks learn that this one is complete
             st.ms_d2h = h->vt.ms_d2h; rc = finish_census(h, need.owes); if (rc) return rc; st.ms_reduce = h->vt.ms_fmt;
             break;
@@ -2315,7 +2452,7 @@ static std::string json_quote(const std::string& s) {      // writeStringJson (f
     }
     return q + "\"";
 }
-static int run_view_lines(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb cb, void* user, TextFormat fmt) {
+static int run_view_lines(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb cb, void* user, TextFormat fmt, const char* header_text = nullptr, size_t header_len = 0) {
     if (!h) return BDEPTH_ERR_ARG;
     if (!o || (o->n_regions && !o->regions)) return fail(h, BDEPTH_ERR_ARG, "null argument");
     if (o->regions_from < BDEPTH_VIEW_ALL || o->regions_from > BDEPTH_VIEW_POSITIONAL) return fail(h, BDEPTH_ERR_ARG, "regions_from: %d", o->regions_from);
@@ -2323,6 +2460,7 @@ static int run_view_lines(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb
     if (o->n_unmapped) return fail(h, BDEPTH_ERR_ARG, "n_unmapped: give each '*' in its place in the region list (ref_id BDEPTH_VIEW_UNMAPPED)");
     const bool positional = o->regions_from == BDEPTH_VIEW_POSITIONAL;
     if (positional && h->world > 1) return fail(h, BDEPTH_ERR_ARG, "positional regions on several ranks: each region's lines would be split over the ranks (run them on one GPU)");
+    if (fmt == TEXT_BAM && h->world > 1) return fail(h, BDEPTH_ERR_ARG, "view -f bam on several ranks: the member cut of a rank starts from the previous rank's state (run it on one GPU)");
     const size_t nref = h->hdr.ref_len.size();
     int rc = init_device(h); if (rc) return rc;
     auto& V = h->vt;
@@ -2335,13 +2473,26 @@ static int run_view_lines(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb
         if (!all.empty()) CK(cudaMemcpy(V.names.as<uint8_t>() + (nref + 1) * 4, all.data(), all.size(), cudaMemcpyHostToDevice));
         V.tab = SamTab{(const char*)(V.names.as<uint8_t>() + (nref + 1) * 4), V.names.as<uint32_t>(), (int32_t)nref, nullptr};
     }
-    V.cb = cb; V.user = user; V.pend[0] = V.pend[1] = false; V.next = 0; V.fmt = fmt;
+    V.cb = cb; V.user = user; V.pend[0] = V.pend[1] = false; V.next = 0; V.fmt = fmt; V.ms_fmt = V.ms_d2h = 0;
+    bool header_out = fmt != TEXT_BAM;
+    auto bam_header = [&]() -> int {      // BamWriter: BAM_MAGIC, writeSamHeader, writeReferenceSequenceInfo, flushCurrentBlock
+        std::string b("BAM\1", 4);
+        auto put32 = [&](uint32_t v) { for (int i = 0; i < 4; i++) b += (char)(v >> (8 * i)); };
+        put32((uint32_t)header_len); b.append(header_text ? header_text : "", header_len);
+        put32((uint32_t)nref);
+        for (size_t r = 0; r < nref; r++) { const std::string& nm = h->hdr.ref_names[r]; put32((uint32_t)nm.size() + 1); b += nm; b += '\0'; put32((uint32_t)h->hdr.ref_len[r]); }
+        CK(h->vb.stage.ensure(b.size() + 16)); CK(cudaMemcpy(h->vb.stage.p, b.data(), b.size(), cudaMemcpyHostToDevice));
+        h->vb.P = 0; h->vb.cur = 0;
+        header_out = true;
+        return bam_emit_run(h, h->vb.stage.as<uint8_t>(), b.size());
+    };
     auto one_run = [&](const bdepth_region* regs, size_t n, uint32_t n_star, bdepth_stats& acc) -> int {
         std::vector<bdepth_region> plan; bool empty = false;
         int r = view_setup(h, o, regs, n, n_star, plan, &empty); if (r) return r;
+        if (!header_out) { r = bam_header(); if (r) return r; }
         if (empty) { h->st = bdepth_stats{}; return 0; }
         std::swap(h->regions, plan);
-        r = run_pipeline(h, RUN_VIEW_TEXT, nullptr);
+        r = run_pipeline(h, fmt == TEXT_BAM ? RUN_VIEW_BAM : RUN_VIEW_TEXT, nullptr);
         std::swap(h->regions, plan);
         if (r) return r;
         const bdepth_stats& s = h->st;
@@ -2369,12 +2520,27 @@ static int run_view_lines(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb
             if (rc) return rc;
         }
     }
+    if (fmt == TEXT_BAM) {      // the open member, then BGZF_EOF (BgzfOutputStream.close)
+        V.ms_fmt = 0; V.ms_d2h = 0;
+        if (h->vb.P) { rc = bam_emit_run(h, h->vb.carry.as<uint8_t>(), h->vb.P); if (rc) return rc; h->vb.P = 0; }
+        rc = view_text_flush(h); if (rc) return rc;
+        acc.ms_reduce += V.ms_fmt; acc.ms_d2h += V.ms_d2h;
+        static const uint8_t BGZF_EOF[28] = {31, 139, 8, 4, 0, 0, 0, 0, 0, 255, 6, 0, 66, 67, 2, 0, 27, 0, 3, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+        if (cb && cb(user, (const char*)BGZF_EOF, sizeof BGZF_EOF)) return fail(h, BDEPTH_ERR_CALLBACK, "text callback aborted");
+    }
     h->st = acc;
     h->st.ms_total_device = h->st.ms_h2d + h->st.ms_inflate + h->st.ms_scan + h->st.ms_reduce + h->st.ms_d2h;
     return 0;
 }
 int bdepth_run_view_text(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb cb, void* user) { return run_view_lines(h, o, cb, user, TEXT_SAM); }
 int bdepth_run_view_json(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb cb, void* user) { return run_view_lines(h, o, cb, user, TEXT_JSON); }
+int bdepth_run_view_bam(bdepth_t* h, const bdepth_view_opts* o, const char* header_text, size_t header_len, int level, bdepth_text_cb cb, void* user) {
+    if (!h) return BDEPTH_ERR_ARG;
+    if (level < -1 || level > 9) return fail(h, BDEPTH_ERR_ARG, "Compression level must be a number in interval [-1, 9]");
+    if (!header_text && header_len) return fail(h, BDEPTH_ERR_ARG, "null argument");
+    h->vb.level = level;
+    return run_view_lines(h, o, cb, user, TEXT_BAM, header_text, header_len);
+}
 
 int bdepth_ref_has_reads(const bdepth_t* h, int ref) {
     if (ref < 0 || (size_t)ref >= h->hdr.ref_len.size() || h->ref_has_host.empty()) return 0;

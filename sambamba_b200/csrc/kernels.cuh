@@ -25,6 +25,7 @@
 #include "inflate_core.cuh"
 #include "inflate2_core.cuh"
 #include "filter.cuh"
+#include "bgzf_deflate.cuh"
 
 namespace bdk {
 
@@ -1884,6 +1885,110 @@ __global__ void __launch_bounds__(256, 1) k_sam_write(const int64_t* __restrict_
     const unsigned long long base = off[r0];
     for (uint32_t r = r0 + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5); r < r1; r += nw)
         if (len[r]) sam_line<true>(u + rec_off[r], t, out + (off[r] - base), lane);
+}
+
+// ---- sambamba view -f bam: BamSerializer (utils/view/alignmentrangeprocessor.d:108-147) over BamWriter (BioD/bio/std/hts/bam/writer.d).
+// Gather: k_bam_len gives 4 + block_size for each selected read (0 otherwise) and refuses a refID outside -1 / [0, n_ref) as unsigned
+// (writeRecord's enforce); the SAM scan turns the sizes into offsets; k_bam_write copies the reads there with bin = reg2bin(pos, pos +
+// basesCovered) (_recalculate_bin) and the last byte of the read name zeroed (read.d:616: the top byte of tlen when l_read_name is 0).
+constexpr unsigned long long BAM_ERR_REF = 7;      // in the error word next to SAM_ERR_*: "Read reference ID is out of range"
+__global__ void __launch_bounds__(256) k_bam_len(RecordSoA soa, const uint8_t* __restrict__ u, uint32_t R, int64_t own_from, ViewSel vs, uint32_t n_ref,
+                                                 unsigned long long* __restrict__ err, uint32_t* __restrict__ len) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= R) return;
+    uint32_t n = 0;
+    if (view_select(soa, u, r, own_from, vs)) {
+        const uint32_t ref = ldu32(u + soa.off[r]);
+        if (ref != 0xFFFFFFFFu && ref >= n_ref) atomicMax(err, BAM_ERR_REF);
+        n = 4 + ldu32(u + soa.off[r] - 4);
+    }
+    len[r] = n;
+}
+__device__ __forceinline__ uint32_t bam_reg2bin(int32_t beg, int32_t end) {      // bai/bin.d:82-92, in D's wrapping int arithmetic
+    if (end == beg) end = (int32_t)((uint32_t)beg + 1u);
+    end = (int32_t)((uint32_t)end - 1u);
+    if (beg >> 14 == end >> 14) return (uint16_t)(4681 + (beg >> 14));
+    if (beg >> 17 == end >> 17) return (uint16_t)(585 + (beg >> 17));
+    if (beg >> 20 == end >> 20) return (uint16_t)(73 + (beg >> 20));
+    if (beg >> 23 == end >> 23) return (uint16_t)(9 + (beg >> 23));
+    if (beg >> 26 == end >> 26) return (uint16_t)(1 + (beg >> 26));
+    return 0;
+}
+// a warp per record: out + off[r] receives record r (block_size field first)
+__global__ void __launch_bounds__(256) k_bam_write(RecordSoA soa, const uint8_t* __restrict__ u, uint32_t R, const uint32_t* __restrict__ len,
+                                                   const unsigned long long* __restrict__ off, uint8_t* __restrict__ out) {
+    const uint32_t lane = threadIdx.x & 31, nw = gridDim.x * (blockDim.x >> 5);
+    for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < R; r += nw) {
+        const uint32_t n = len[r];
+        if (!n) continue;
+        const uint8_t* s = u + soa.off[r] - 4; uint8_t* d = out + off[r];
+        const uint32_t l_name = s[12], n_cigar = ldu16(s + 16), flag = ldu16(s + 18);
+        uint32_t bc = 0;
+        if (!(flag & 4u)) for (uint32_t i = lane; i < n_cigar; i += 32) { const uint32_t c = ldu32(s + 36 + l_name + 4 * i); if (cig_rcons(c & 15)) bc += c >> 4; }
+        for (int sh = 16; sh; sh >>= 1) bc += __shfl_xor_sync(0xFFFFFFFFu, bc, sh);
+        const int32_t pos = (int32_t)ldu32(s + 8);
+        const uint32_t bin = bam_reg2bin(pos, (int32_t)((uint32_t)pos + bc));
+        const uint32_t zero_at = 35 + l_name;
+        for (uint32_t j = lane; j < n; j += 32) d[j] = j == 14 ? (uint8_t)bin : j == 15 ? (uint8_t)(bin >> 8) : j == zero_at ? (uint8_t)0 : s[j];
+    }
+}
+// Member cut (BamWriter.writeRecord + BgzfOutputStream.writeBlock): a record opens a new member when it does not fit behind the bytes written
+// since the last explicit flush (cur); a member also closes whenever its buffer reaches BGZF_BLOCK bytes.  So the stream falls into groups,
+// each a greedy run of records from a record that did not fit, and a group of n bytes is ceil(n / BGZF_BLOCK) members.  Per sub-batch, with
+// the records' offsets off[] (total bytes) and P carried bytes of the open member in front of them in the stage:
+//   - nx[i]: the record after the group that record i would open (k_bam_next, a binary search); nx[R] = R;
+//   - the chain of group starts: s0 (the first record the carried group cannot take, k_bam_start), then nx[s0], ... -- marked by pointer
+//     doubling: jump tables J_k = nx^(2^k) (k_bam_jump), then from the top level down each marked record marks J_k of itself (k_bam_mark);
+//   - k_bam_members: entry 0 is the carried group, entry i + 1 a group opened at record i; the open group's full members go out now, its
+//     rest (P' bytes) and cur' are carried on.
+__device__ __forceinline__ unsigned long long bam_off(const unsigned long long* off, uint32_t k, uint32_t R, unsigned long long total) { return k < R ? off[k] : total; }
+__global__ void k_bam_next(const unsigned long long* __restrict__ off, uint32_t R, unsigned long long total, uint32_t* __restrict__ nx) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= R; i += gridDim.x * blockDim.x) {
+        if (i == R) { nx[R] = R; continue; }
+        const unsigned long long o = off[i];
+        uint32_t a = i, b = R;                                     // the last k with off[k] - off[i] <= BGZF_BLOCK
+        while (a < b) { const uint32_t mid = (a + b + 1) >> 1; if (bam_off(off, mid, R, total) - o <= BGZF_BLOCK) a = mid; else b = mid - 1; }
+        nx[i] = a > i ? a : i + 1;
+    }
+}
+__global__ void k_bam_start(const unsigned long long* __restrict__ off, uint32_t R, unsigned long long total, unsigned long long cur, uint8_t* __restrict__ mark, uint32_t* __restrict__ s0) {
+    uint32_t a = 0, b = R;                                         // the first j with cur + off[j + 1] > BGZF_BLOCK
+    while (a < b) { const uint32_t mid = (a + b) >> 1; if (cur + bam_off(off, mid + 1, R, total) > BGZF_BLOCK) b = mid; else a = mid + 1; }
+    *s0 = a; mark[a] = 1;
+}
+__global__ void k_bam_jump(const uint32_t* __restrict__ j, uint32_t* __restrict__ j2, uint32_t R) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= R; i += gridDim.x * blockDim.x) j2[i] = j[j[i]];
+}
+__global__ void k_bam_mark(const uint32_t* __restrict__ j, uint8_t* mark, uint32_t R) {      // (a mark set during the pass is a chain record too)
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < R; i += gridDim.x * blockDim.x) if (mark[i]) mark[j[i]] = 1;
+}
+// entry e's group [A, B) in the stage, and whether it is still open at the end of the sub-batch
+__device__ __forceinline__ uint32_t bam_group(uint32_t e, const unsigned long long* off, uint32_t R, unsigned long long total, const uint32_t* nx, const uint8_t* mark,
+                                              uint32_t s0, uint32_t P, unsigned long long* A, unsigned long long* B, bool* open) {
+    const unsigned long long E = P + total;
+    if (e == 0) { *A = 0; *open = s0 >= R; *B = *open ? E : P + off[s0]; }
+    else {
+        const uint32_t i = e - 1;
+        if (!mark[i]) return 0;
+        *A = P + off[i]; *open = nx[i] >= R; *B = *open ? E : P + off[nx[i]];
+    }
+    const unsigned long long n = *B - *A;
+    return (uint32_t)(*open ? n / BGZF_BLOCK : (n + BGZF_BLOCK - 1) / BGZF_BLOCK);
+}
+// WRITE = false: cnt[e] = the members entry e closes; true: their stage offsets and lengths at base[e], and the open group's rest into ctl:
+// ctl[0] = P' (its bytes not yet in a member), ctl[1] = cur' (BamWriter's _current_size)
+template <bool WRITE>
+__global__ void k_bam_members(const unsigned long long* __restrict__ off, uint32_t R, unsigned long long total, const uint32_t* __restrict__ nx, const uint8_t* __restrict__ mark,
+                              const uint32_t* __restrict__ s0p, uint32_t P, unsigned long long cur, uint32_t* __restrict__ cnt, const unsigned long long* __restrict__ base,
+                              unsigned long long* __restrict__ m_off, uint32_t* __restrict__ m_len, unsigned long long* __restrict__ ctl) {
+    const uint32_t s0 = *s0p;
+    for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e <= R; e += gridDim.x * blockDim.x) {
+        unsigned long long A = 0, B = 0; bool open = false;
+        const uint32_t c = bam_group(e, off, R, total, nx, mark, s0, P, &A, &B, &open);
+        if (!WRITE) { cnt[e] = c; continue; }
+        for (uint32_t k = 0; k < c; k++) { const unsigned long long a = A + (unsigned long long)k * BGZF_BLOCK; m_off[base[e] + k] = a; m_len[base[e] + k] = (uint32_t)min(B - a, (unsigned long long)BGZF_BLOCK); }
+        if (open && (e == 0 || mark[e - 1])) { ctl[0] = (B - A) % BGZF_BLOCK; ctl[1] = e == 0 ? cur + total : total - off[e - 1]; }
+    }
 }
 
 // ---- sambamba view -f json: the JSON record of a read, BamRead.toJson (read.d:768-830) plus '\n' (chunkToFormat!'j',

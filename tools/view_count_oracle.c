@@ -21,10 +21,12 @@
  * its escape table, writeFloatJson (%g, +-1.0e+1024 for +-inf, null for NaN) and itoa (format.d:66-87,196-270); its refusals are the SAM line's.
  * -v is a literal C statement of BioD's isValid (bio/std/hts/bam/validation/alignment.d:138-562), applied in view_main's filter chain: after
  * SubsampleFilter, before FlagBitFilter and -F, and before BedFilter; where its tag walk throws or reads past the record, the run fails.
- * Library: view_count_oracle(), view_text_oracle(), view_json_oracle(), view_text_oracle_free(), view_count_oracle_hash(),
+ * `view -f bam` is a literal C statement of BamWriter over BgzfOutputStream (writeRecord's member cut, writeBlock's fill-and-flush, the header
+ * and reference list, _recalculate_bin, the zeroed last name byte) with each member made by bgzfCompress's zlib call (view_bam_oracle()).
+ * Library: view_count_oracle(), view_text_oracle(), view_json_oracle(), view_bam_oracle(), view_bam_oracle_member(), view_text_oracle_free(), view_count_oracle_hash(),
  * view_count_oracle_error(), view_count_oracle_set_valid() (-v for the calls that follow), view_valid_oracle() (one record).  With -DORACLE_MAIN
  * also a CLI:
- *   view_count_oracle view [-c] [-v] [-f sam|json] [--num-filter=I1/I2] [-s FRAC] [--subsampling-seed=SEED] [-L BED] in.bam [region ...]
+ *   view_count_oracle view [-c] [-v] [-f sam|json|bam] [-l LEVEL] [--num-filter=I1/I2] [-s FRAC] [--subsampling-seed=SEED] [-L BED] in.bam [region ...]
  * which prints the count as `sambamba view -c` does, or without -c the SAM lines or JSON records (no header), or "sambamba-view: <msg>" and exit
  * code 1 for the errors it restates. */
 #include <ctype.h>
@@ -108,7 +110,11 @@ uint64_t view_count_oracle_hash(const uint8_t* name, size_t len, uint64_t seed) 
 typedef struct { uint32_t ref, start, end; } Reg;
 
 /* Where selected reads go: counted, or formatted as SAM lines into a growing buffer. */
-typedef struct { int text, json; uint64_t cnt; char* buf; size_t len, cap; int err; } Out;
+/* BamWriter (BioD/bio/std/hts/bam/writer.d) over BgzfOutputStream (bio/core/bgzf/outputstream.d), restated literally for `view -f bam`: the
+ * uncompressed stream, and the size of every member in the order flushCurrentBlock writes them. */
+#define BGZF_BLOCK_SIZE 0xFF00u
+typedef struct { uint8_t* raw; size_t len, cap; uint32_t* ms; size_t nm, mcap; size_t buf_cur /* BgzfOutputStream._current_size */; size_t cur /* BamWriter._current_size */; int n_ref; } BamOut;
+typedef struct { int text, json; uint64_t cnt; char* buf; size_t len, cap; int err; BamOut* bam; } Out;
 static void out_put(Out* o, const void* s, size_t n) {
     if (o->len + n > o->cap) { o->cap = (o->len + n) * 2 + 4096; o->buf = realloc(o->buf, o->cap); }
     memcpy(o->buf + o->len, s, n); o->len += n;
@@ -301,7 +307,58 @@ static int json_line(const Bam* b, const Rec* x, Out* o) {
     return 0;
 }
 
+static void bgzf_flush_current_block(BamOut* w) {                           /* outputstream.d flushCurrentBlock: an empty member is never written */
+    if (w->buf_cur == 0) return;
+    if (w->nm == w->mcap) { w->mcap = w->mcap * 2 + 16; w->ms = realloc(w->ms, w->mcap * sizeof(uint32_t)); }
+    w->ms[w->nm++] = (uint32_t)w->buf_cur;
+    w->buf_cur = 0;
+}
+static void bgzf_write_block(BamOut* w, const void* buf, size_t size) {     /* outputstream.d writeBlock, _buffer.length = BGZF_BLOCK_SIZE */
+    if (w->len + size > w->cap) { w->cap = (w->len + size) * 2 + 65536; w->raw = realloc(w->raw, w->cap); }
+    memcpy(w->raw + w->len, buf, size); w->len += size;
+    if (size + w->buf_cur >= BGZF_BLOCK_SIZE) {
+        size_t data = size;
+        while (data + w->buf_cur >= BGZF_BLOCK_SIZE) {
+            const size_t room = BGZF_BLOCK_SIZE - w->buf_cur;
+            data -= room;
+            w->buf_cur = BGZF_BLOCK_SIZE;
+            bgzf_flush_current_block(w);
+        }
+        w->buf_cur = data;
+    } else w->buf_cur += size;
+}
+static void bam_put32(BamOut* w, uint32_t v) { uint8_t t[4] = {(uint8_t)v, (uint8_t)(v >> 8), (uint8_t)(v >> 16), (uint8_t)(v >> 24)}; bgzf_write_block(w, t, 4); }
+static uint16_t reg2bin(int32_t beg, int32_t end) {                         /* bai/bin.d:82-92 (D's int arithmetic wraps) */
+    if (end == beg) end = (int32_t)((uint32_t)beg + 1u);
+    end = (int32_t)((uint32_t)end - 1u);
+    if (beg >> 14 == end >> 14) return (uint16_t)(((1 << 15) - 1) / 7 + (beg >> 14));
+    if (beg >> 17 == end >> 17) return (uint16_t)(((1 << 12) - 1) / 7 + (beg >> 17));
+    if (beg >> 20 == end >> 20) return (uint16_t)(((1 << 9) - 1) / 7 + (beg >> 20));
+    if (beg >> 23 == end >> 23) return (uint16_t)(((1 << 6) - 1) / 7 + (beg >> 23));
+    if (beg >> 26 == end >> 26) return (uint16_t)(((1 << 3) - 1) / 7 + (beg >> 26));
+    return 0;
+}
+/* BamWriter.writeRecord (writer.d) with BamRead._recalculate_bin and BamRead.write (read.d:613-630, 1028-1030) */
+static int bam_write_record(BamOut* w, const Rec* x, Out* o) {
+    if (!(x->ref == -1 || (uint32_t)x->ref < (uint32_t)w->n_ref)) return sam_fail(o, "Read reference ID is out of range");
+    uint8_t* chunk = malloc(x->bs ? x->bs : 1); memcpy(chunk, x->p, x->bs);
+    const uint32_t bc = x->flag & 4 ? 0u : (uint32_t)x->bc;                   /* basesCovered: 0 for an unmapped read */
+    const uint16_t bin = reg2bin(x->pos, (int32_t)((uint32_t)x->pos + bc));
+    chunk[10] = (uint8_t)bin; chunk[11] = (uint8_t)(bin >> 8);
+    const size_t read_size = 4 + (size_t)x->bs;                               /* size_in_bytes */
+    if (read_size + w->cur > BGZF_BLOCK_SIZE) bgzf_flush_current_block(w);
+    const uint32_t cigar_offset = 32 + x->l_name, tags_offset = cigar_offset + 4 * (rd32(x->p + 12) & 0xFFFF) + (((uint32_t)rd32(x->p + 16) + 1) / 2) + rd32(x->p + 16);
+    const uint32_t tags_at = tags_offset < x->bs ? tags_offset : x->bs;
+    bam_put32(w, x->bs);                                                       /* writeInteger(cast(int)_chunk.length) */
+    chunk[cigar_offset - 1] = 0;                                               /* _chunk[_cigar_offset - 1] = 0 */
+    bgzf_write_block(w, chunk, tags_at);                                       /* writeByteArray(_chunk[0 .. _tags_offset]) */
+    bgzf_write_block(w, chunk + tags_at, x->bs - tags_at);                    /* writeTags */
+    free(chunk);
+    if (read_size + w->cur > BGZF_BLOCK_SIZE) w->cur = read_size; else w->cur += read_size;
+    return 0;
+}
 static void emit(const Bam* b, const Rec* x, Out* o) {
+    if (o->bam) { if (!o->err) bam_write_record(o->bam, x, o); return; }
     if (!o->text) { o->cnt++; return; }
     if (!o->err) (o->json ? json_line : sam_line)(b, x, o);
 }
@@ -578,6 +635,62 @@ int view_json_oracle(const char* path, unsigned flag_set, unsigned flag_unset, i
 }
 void view_text_oracle_free(char* text) { free(text); }
 
+/* bgzfCompress (bio/core/bgzf/compress.d) of one member with the system zlib: BLOCK_HEADER_START, BSIZE - 1, deflateInit2(level, Z_DEFLATED, -15,
+ * 8, Z_DEFAULT_STRATEGY) with Z_FINISH, CRC32, ISIZE.  Returns the member's length in out (65536 bytes at least). */
+static size_t bgzf_compress(const uint8_t* in, size_t n, int level, uint8_t* out) {
+    static const uint8_t hs[16] = {31, 139, 8, 4, 0, 0, 0, 0, 0, 255, 6, 0, 66, 67, 2, 0};
+    memcpy(out, hs, 16);
+    z_stream zs; memset(&zs, 0, sizeof zs);
+    zs.next_in = (Bytef*)in; zs.avail_in = (uInt)n; zs.next_out = out + 18; zs.avail_out = 65536 - 18 - 8;
+    if (deflateInit2(&zs, level, Z_DEFLATED, -15, 8, Z_DEFAULT_STRATEGY) != Z_OK || deflate(&zs, Z_FINISH) != Z_STREAM_END) return 0;
+    const size_t total = zs.total_out + 18 + 8;
+    deflateEnd(&zs);
+    out[16] = (uint8_t)(total - 1); out[17] = (uint8_t)((total - 1) >> 8);
+    const uint32_t crc = (uint32_t)crc32(0, in, (uInt)n);
+    for (int i = 0; i < 4; i++) { out[total - 8 + i] = (uint8_t)(crc >> (8 * i)); out[total - 4 + i] = (uint8_t)(n >> (8 * i)); }
+    return total;
+}
+size_t view_bam_oracle_member(const uint8_t* in, size_t n, int level, uint8_t* out) { return bgzf_compress(in, n, level, out); }
+/* `sambamba view -f bam` (view.d:380-386, BamSerializer): the uncompressed stream (*raw), the sizes of its members (*ms, *nm) and the finished
+ * file, members by the system zlib plus BGZF_EOF (*file).  Selection arguments as view_text_oracle; header_text: the header text given to
+ * writeSamHeader; the reference list is the file's.  Each output is freed with view_text_oracle_free(). */
+int view_bam_oracle(const char* path, unsigned flag_set, unsigned flag_unset, int subsample, uint64_t threshold, uint64_t seed,
+                    int mode, const uint32_t* regs, size_t nreg, const char* header_text, size_t header_len, int level,
+                    uint8_t** raw, size_t* raw_len, uint32_t** ms, size_t* nm, uint8_t** file, size_t* file_len) {
+    Bam b; g_err[0] = 0;
+    if (level < -1 || level > 9) { snprintf(g_err, sizeof g_err, "Compression level must be a number in interval [-1, 9]"); return -1; }
+    if (bam_load(path, &b)) { bam_free(&b); return -1; }
+    BamOut w; memset(&w, 0, sizeof w); w.n_ref = b.n_ref;
+    bgzf_write_block(&w, "BAM\1", 4);                                          /* the constructor: writeString(BAM_MAGIC) */
+    bam_put32(&w, (uint32_t)header_len); bgzf_write_block(&w, header_text, header_len);      /* writeSamHeader */
+    bam_put32(&w, (uint32_t)b.n_ref);                                          /* writeReferenceSequenceInfo */
+    {
+        size_t o = 8 + rd32(b.u + 4) + 4;
+        for (int r = 0; r < b.n_ref; r++) {
+            const uint32_t ln = rd32(b.u + o); const size_t nl = strlen(b.names[r]);
+            bam_put32(&w, (uint32_t)(nl + 1)); bgzf_write_block(&w, b.names[r], nl); { uint8_t z = 0; bgzf_write_block(&w, &z, 1); }
+            bam_put32(&w, rd32(b.u + o + 4 + ln));
+            o += 8 + ln;
+        }
+    }
+    bgzf_flush_current_block(&w);
+    Out out = {0}; out.bam = &w;
+    const int rc = view_stream(&b, flag_set, flag_unset, subsample, threshold, seed, mode, regs, nreg, 0, &out);
+    bam_free(&b);
+    if (rc) { free(w.raw); free(w.ms); return -1; }
+    bgzf_flush_current_block(&w);                                              /* close: flush, then the EOF block */
+    uint8_t* f = malloc(w.nm * 65536 + 28); size_t fl = 0, at = 0;
+    for (size_t i = 0; i < w.nm; i++) {
+        const size_t k = bgzf_compress(w.raw + at, w.ms[i], level, f + fl);
+        if (!k) { snprintf(g_err, sizeof g_err, "zlib failed"); free(f); free(w.raw); free(w.ms); return -1; }
+        fl += k; at += w.ms[i];
+    }
+    static const uint8_t eof[28] = {31, 139, 8, 4, 0, 0, 0, 0, 0, 255, 6, 0, 66, 67, 2, 0, 27, 0, 3, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    memcpy(f + fl, eof, 28); fl += 28;
+    *raw = w.raw; *raw_len = w.len; *ms = w.ms; *nm = w.nm; *file = f; *file_len = fl;
+    return 0;
+}
+
 #ifdef ORACLE_MAIN
 static int die(const char* m) { fprintf(stderr, "sambamba-view: %s\n", m); return 1; }
 static int conv_u(const char* s, unsigned long long maxv, const char* type, unsigned long long* v) {
@@ -609,7 +722,7 @@ static void parse_region(const char* s, char* ref, size_t cap, uint32_t* beg, ui
 }
 int main(int argc, char** argv) {
     if (argc < 2 || strcmp(argv[1], "view")) { fprintf(stderr, "usage: view_count_oracle view [-c] [options] in.bam [region ...]\n"); return 1; }
-    unsigned long long fs = 0, fu = 0, seed = 0; double frac = NAN; const char* bed = NULL; int count = 0, json = 0;
+    unsigned long long fs = 0, fu = 0, seed = 0; double frac = NAN; const char* bed = NULL; int count = 0, json = 0, bam = 0, level = -1;
     const char* pos_args[4096]; int npos = 0;
     for (int i = 2; i < argc; i++) {
         const char* a = argv[i];
@@ -625,9 +738,10 @@ int main(int argc, char** argv) {
         else if (!strcmp(a, "-L") && i + 1 < argc) bed = argv[++i];
         else if (!strcmp(a, "-f") && i + 1 < argc) {
             const char* f = argv[++i];
-            if (strcmp(f, "sam") && strcmp(f, "json")) return die("output format must be sam or json here");
-            json = !strcmp(f, "json");
+            if (strcmp(f, "sam") && strcmp(f, "json") && strcmp(f, "bam")) return die("output format must be sam, json or bam here");
+            json = !strcmp(f, "json"); bam = !strcmp(f, "bam");
         }
+        else if (!strcmp(a, "-l") && i + 1 < argc) level = atoi(argv[++i]);
         else if (npos < 4096) pos_args[npos++] = a;
     }
     if (npos < 1) { fprintf(stderr, "usage: view_count_oracle view [-c] [options] in.bam [region ...]\n"); return 1; }
@@ -678,6 +792,15 @@ int main(int argc, char** argv) {
         }
     }
     bam_free(&b);
+    if (!count && bam) {      /* the file, with the input's own header text */
+        if (mode == 2 && !n) mode = 0;
+        Bam hb; if (bam_load(pos_args[0], &hb)) { bam_free(&hb); return die(g_err); }
+        const uint32_t lt = rd32(hb.u + 4); char* ht = malloc(lt + 1); memcpy(ht, hb.u + 8, lt); bam_free(&hb);
+        uint8_t *raw = NULL, *file = NULL; uint32_t* ms = NULL; size_t rl = 0, nm = 0, fl = 0;
+        if (view_bam_oracle(pos_args[0], (unsigned)fs, (unsigned)fu, sub, thr, seed, mode, regs, n, ht, lt, level, &raw, &rl, &ms, &nm, &file, &fl)) { free(ht); free(regs); return die(g_err); }
+        fwrite(file, 1, fl, stdout); free(raw); free(ms); free(file); free(ht); free(regs);
+        return 0;
+    }
     if (!count) {
         if (mode == 2 && !n) mode = 0;
         char* text = NULL; size_t len = 0;
