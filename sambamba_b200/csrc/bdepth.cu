@@ -242,21 +242,25 @@ struct bdepth {
     ViewSel vsel{}; DevBuf vc, vc_reg, vc_prog; uint64_t vc_host[2] = {};
     // ---- view -v: k_view_valid's status of each record of the sub-batch
     bool view_valid = false; DevBuf vv;
-    // ---- view's SAM lines (bdepth_run_view_text): per sub-batch the line lengths, their offsets and the piece cuts; two text slots on the device
-    // and their pinned host copies (one is handed to the callback while the next piece is written and copied); timings of the run
-    struct ViewText {
+    // ---- view's output (SAM, JSON, BAM): the piece cuts, two slots on the device and their pinned host copies (the callback gets one while the
+    // next piece is written and copied into the other), and the run's timings
+    struct SlotRing {
         bdepth_text_cb cb = nullptr; void* user = nullptr;
-        DevBuf names, len, off, tiles, ctl, cut_r, cut_o, slot[2];
+        DevBuf cut_r, cut_o, slot[2];
         char* host = nullptr; size_t cap = 0;          // bytes per slot (device and host)
         bool pend[2] = {false, false}; size_t pend_len[2] = {0, 0}; int next = 0;
-        uint64_t issued = 0;                           // bytes handed to the D2H in the current pipeline run
+        uint64_t issued = 0;                           // bytes of output handed out in the current pipeline run (each format counts its own)
         float ms_fmt = 0, ms_d2h = 0;
+    } ring;
+    // ---- view's SAM and JSON lines (bdepth_run_view_text / _json): per sub-batch the line lengths and their offsets
+    struct ViewText {
+        DevBuf names, len, off, tiles, ctl;
         SamTab tab{};                                  // the reference names on the device, as the format prints them (ctl is set per sub-batch)
         TextFormat fmt = TEXT_SAM;                     // which line view_text_sub formats: SAM (bdepth_run_view_text) or JSON (bdepth_run_view_json)
     } vt;
     // ---- view -f bam (bdepth_run_view_bam): the stage of a sub-batch (the open member's bytes carried in front of the gathered reads), the member
     // cut's tables, the members' compressed bytes (BGZF_SLOT apart), and the cut state that passes from one sub-batch and run to the next:
-    // P bytes of the open member in `carry`, cur = BamWriter._current_size.  Delivery goes through vt's slots.
+    // P bytes of the open member in `carry`, cur = BamWriter._current_size.  Delivery goes through the ring.
     struct ViewBam {
         DevBuf stage, carry, len, off, tiles, ctiles, ctl, nx, mark, cnt, base, m_off, m_len, comp, clen, coff, tok;
         uint32_t P = 0; unsigned long long cur = 0; int level = -1;
@@ -715,105 +719,45 @@ struct RunOut {                    // optional sinks for the kernel-level entry 
 
 __global__ void k_fill_u32(uint32_t* p, uint32_t v, uint64_t n) { uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; if (i < n) p[i] = v; }
 
-// ---- view's SAM lines (RUN_VIEW_TEXT).  Per sub-batch, while its records are still in the inflate buffer: k_sam_len measures the line of every
-// selected record, a device-wide scan turns the lengths into offsets, one small copy brings the total, the longest line and the error word down,
-// and k_sam_cut cuts the records into pieces of about VIEW_TEXT_PIECE bytes of text (a piece always holds whole lines, so a slot holds a piece plus
-// the longest line).  Each piece is written by k_sam_write into a device slot and copied into pinned memory on the D2H stream; the callback
-// gets a slot while the next piece is written and copied into the other.
+// ---- view's output ring (SAM, JSON and BAM).  A sub-batch's output is n items (lines or members) at device offsets off, total bytes in all;
+// k_sam_cut cuts them into pieces of whole items of about ring_piece() bytes.  Each piece is written into a device slot on the main stream and
+// copied into pinned memory on the D2H stream; the callback gets a slot while the next piece is written and copied into the other.
+// Events, per slot s: EV_RING_BEGIN + s .. EV_RING_WRITTEN + s around the write (ms_fmt), EV_RING_COPIED + s after the copy (ms_d2h); and
+// EV_FMT_BEGIN .. EV_FMT_END around a sub-batch's work before its pieces (ms_fmt).
 constexpr uint64_t VIEW_TEXT_PIECE = 64ull << 20;     // capped by the batch size (bdepth_set_tuning), so that small batches make many pieces
-const char* sam_err_msg(unsigned long long c) {
-    switch (c) {
-        case SAM_ERR_REF: return "a record's reference ID lies outside [-1, n_ref): no RNAME to print (the reference indexes its reference list out of bounds)";
-        case SAM_ERR_MATE_REF: return "a record's mate reference ID lies outside [-1, n_ref): no RNEXT to print (the reference indexes its reference list out of bounds)";
-        case SAM_ERR_TAG_TYPE: return "unknown tag type in a record's auxiliary data (UnknownTagTypeException)";
-        case SAM_ERR_B_TYPE: return "unknown element type of a B array in a record's auxiliary data (UnknownTagTypeException)";
-        case SAM_ERR_NO_NUL: return "a Z or H tag value without its terminating NUL";
-        default: return "a record's fields, a tag or a B array run past the record's block_size";
-    }
-}
-int view_text_deliver(bdepth* h, int slot) {
-    auto& V = h->vt;
-    if (!V.pend[slot]) return 0;
-    CK(cudaEventSynchronize(h->ev[26 + slot])); V.pend[slot] = false;
-    float t = 0; CK(cudaEventElapsedTime(&t, h->ev[28 + slot], h->ev[24 + slot])); V.ms_fmt += t;
-    CK(cudaEventElapsedTime(&t, h->ev[24 + slot], h->ev[26 + slot])); V.ms_d2h += t;
-    if (V.cb && V.pend_len[slot] && V.cb(V.user, V.host + (size_t)slot * V.cap, V.pend_len[slot])) return fail(h, BDEPTH_ERR_CALLBACK, "text callback aborted");
+constexpr int EV_RING_WRITTEN = 24, EV_RING_COPIED = 26, EV_RING_BEGIN = 28, EV_FMT_BEGIN = 30, EV_FMT_END = 31;
+uint64_t ring_piece(const bdepth* h) { return std::max<uint64_t>(1, std::min<uint64_t>(VIEW_TEXT_PIECE, h->batch_u)); }
+int ring_deliver(bdepth* h, int s) {      // slot s's piece to the callback, once its copy is done
+    auto& Q = h->ring;
+    if (!Q.pend[s]) return 0;
+    CK(cudaEventSynchronize(h->ev[EV_RING_COPIED + s])); Q.pend[s] = false;
+    float t = 0; CK(cudaEventElapsedTime(&t, h->ev[EV_RING_BEGIN + s], h->ev[EV_RING_WRITTEN + s])); Q.ms_fmt += t;
+    CK(cudaEventElapsedTime(&t, h->ev[EV_RING_WRITTEN + s], h->ev[EV_RING_COPIED + s])); Q.ms_d2h += t;
+    if (Q.cb && Q.pend_len[s] && Q.cb(Q.user, Q.host + (size_t)s * Q.cap, Q.pend_len[s])) return fail(h, BDEPTH_ERR_CALLBACK, "text callback aborted");
     return 0;
 }
-int view_text_flush(bdepth* h) { int rc = view_text_deliver(h, h->vt.next); if (!rc) rc = view_text_deliver(h, h->vt.next ^ 1); return rc; }
-// view -v: k_view_valid over the sub-batch's R records, and vs (the run's selection) pointed at its statuses, refusals going to *err
-int launch_view_valid(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R, int64_t own_from, unsigned long long* err, ViewSel& vs) {
-    CK(h->vv.ensure(R));
-    BD_LAUNCH((unsigned)std::min<uint64_t>((R + VV_WARPS - 1) / VV_WARPS, 8192), VV_WARPS * 32, 0, h->s_main, k_view_valid)(soa, u0, R, own_from, h->vv.as<uint8_t>());
-    CK(cudaGetLastError()); h->st.gpu_launches++;
-    vs.vstat = h->vv.as<uint8_t>(); vs.verr = err;
+int ring_flush(bdepth* h) { int rc = ring_deliver(h, h->ring.next); if (!rc) rc = ring_deliver(h, h->ring.next ^ 1); return rc; }
+int ring_reserve(bdepth* h, size_t need, size_t size) {      // slots of at least `need` bytes: else hand out what is pending, reallocate both at `size`
+    auto& Q = h->ring;
+    if (need <= Q.cap) return 0;
+    int rc = ring_flush(h); if (rc) return rc;
+    if (Q.host) cudaFreeHost(Q.host);
+    Q.host = nullptr; Q.cap = 0;
+    CK(cudaMallocHost((void**)&Q.host, 2 * size)); CK(Q.slot[0].ensure(size)); CK(Q.slot[1].ensure(size));
+    Q.cap = size;
     return 0;
 }
-int view_text_sub(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R, int64_t own_from) {
-    auto& V = h->vt; cudaStream_t sm = h->s_main;
-    const uint32_t n_tiles = (R + SAM_SCAN_TILE - 1) / SAM_SCAN_TILE;
-    const size_t toff_at = ((size_t)n_tiles * 4 + 7) / 8 * 8;
-    CK(V.len.ensure((size_t)R * 4)); CK(V.off.ensure((size_t)R * 8)); CK(V.tiles.ensure(toff_at + (size_t)n_tiles * 8)); CK(V.ctl.ensure(32));
-    uint32_t* len = V.len.as<uint32_t>(); unsigned long long* off = V.off.as<unsigned long long>();
-    uint32_t* tsum = V.tiles.as<uint32_t>(); unsigned long long* toff = (unsigned long long*)(V.tiles.as<uint8_t>() + toff_at);
-    SamTab t = V.tab; t.ctl = V.ctl.as<unsigned long long>();
-    CK(cudaMemsetAsync(t.ctl, 0, 24, sm));
-    CK(cudaEventRecord(h->ev[30], sm));
-    ViewSel vs = h->vsel;
-    if (h->view_valid) { int rc = launch_view_valid(h, soa, u0, R, own_from, t.ctl + 2, vs); if (rc) return rc; }      // refusals share the lines' error word
-    if (V.fmt == TEXT_JSON) BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_json_len)(soa, u0, R, own_from, vs, t, len);
-    else BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_sam_len)(soa, u0, R, own_from, vs, t, len);
-    BD_LAUNCH(n_tiles, 256, 0, sm, k_sam_tile_sum)(len, R, tsum);
-    BD_LAUNCH(1, 1024, 0, sm, k_text_scan)(tsum, n_tiles, toff, t.ctl);
-    BD_LAUNCH(n_tiles, 256, 0, sm, k_sam_scan_apply)(len, R, toff, off);
-    CK(cudaGetLastError()); h->st.gpu_launches += 4;
-    CK(cudaEventRecord(h->ev[31], sm));
-    unsigned long long c[3]; CK(cudaMemcpyAsync(c, t.ctl, 24, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
-    { float tm = 0; CK(cudaEventElapsedTime(&tm, h->ev[30], h->ev[31])); V.ms_fmt += tm; }
-    if (c[2]) return fail(h, BDEPTH_ERR_FORMAT, "%s", sam_err_msg(c[2]));
-    const uint64_t total = c[0];
-    if (!total) return 0;
-    const uint64_t piece = std::max<uint64_t>(1, std::min<uint64_t>(VIEW_TEXT_PIECE, h->batch_u));
-    if (piece + c[1] > V.cap) {      // a slot holds a piece and its longest line: grow both, after handing out what is pending in them
-        int rc = view_text_flush(h); if (rc) return rc;
-        if (V.host) { cudaFreeHost(V.host); V.host = nullptr; }
-        V.cap = 0;
-        const size_t need = piece + std::max<uint64_t>(c[1], piece);
-        CK(cudaMallocHost((void**)&V.host, 2 * need)); CK(V.slot[0].ensure(need)); CK(V.slot[1].ensure(need));
-        V.cap = need;
-    }
-    const uint32_t n_cuts = (uint32_t)((total + piece - 1) / piece) + 1;
-    CK(V.cut_r.ensure((size_t)n_cuts * 4)); CK(V.cut_o.ensure((size_t)n_cuts * 8));
-    BD_LAUNCH((n_cuts + 255) / 256, 256, 0, sm, k_sam_cut)(off, R, total, piece, n_cuts, V.cut_r.as<uint32_t>(), V.cut_o.as<unsigned long long>());
-    CK(cudaGetLastError()); h->st.gpu_launches++;
-    std::vector<uint32_t> cr(n_cuts); std::vector<unsigned long long> co(n_cuts);
-    CK(cudaMemcpyAsync(cr.data(), V.cut_r.p, (size_t)n_cuts * 4, cudaMemcpyDeviceToHost, sm)); CK(cudaMemcpyAsync(co.data(), V.cut_o.p, (size_t)n_cuts * 8, cudaMemcpyDeviceToHost, sm));
+// the end of the span begun at EV_FMT_BEGIN: record it, bring n bytes at src down to dst, wait for the main stream, and count the span in ms_fmt
+int fmt_span_end(bdepth* h, void* dst = nullptr, const void* src = nullptr, size_t n = 0) {
+    cudaStream_t sm = h->s_main;
+    CK(cudaEventRecord(h->ev[EV_FMT_END], sm));
+    if (n) CK(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, sm));
     CK(cudaStreamSynchronize(sm));
-    for (uint32_t j = 0; j + 1 < n_cuts; j++) {
-        const uint32_t r0 = cr[j], r1 = j + 2 == n_cuts ? R : cr[j + 1];
-        const uint64_t bytes = (j + 2 == n_cuts ? total : co[j + 1]) - co[j];
-        if (!bytes) continue;
-        const int s = V.next;
-        int rc = view_text_deliver(h, s); if (rc) return rc;      // the slot's previous piece must be consumed before reuse
-        CK(cudaEventRecord(h->ev[28 + s], sm));
-        const unsigned grid = (unsigned)std::min<uint64_t>((r1 - r0 + 7) / 8, 8192);
-        if (V.fmt == TEXT_JSON) BD_LAUNCH(grid, 256, 0, sm, k_json_write)(soa.off, u0, r0, r1, len, off, t, V.slot[s].as<char>());
-        else BD_LAUNCH(grid, 256, 0, sm, k_sam_write)(soa.off, u0, r0, r1, len, off, t, V.slot[s].as<char>());
-        CK(cudaGetLastError()); h->st.gpu_launches++;
-        CK(cudaEventRecord(h->ev[24 + s], sm));
-        CK(cudaStreamWaitEvent(h->s_d2h, h->ev[24 + s], 0));
-        CK(cudaMemcpyAsync(V.host + (size_t)s * V.cap, V.slot[s].p, bytes, cudaMemcpyDeviceToHost, h->s_d2h));
-        CK(cudaEventRecord(h->ev[26 + s], h->s_d2h));
-        V.pend[s] = true; V.pend_len[s] = bytes; V.issued += bytes; V.next = s ^ 1;
-        rc = view_text_deliver(h, s ^ 1); if (rc) return rc;     // hand out the previous piece while this one is in flight
-    }
+    float tm = 0; CK(cudaEventElapsedTime(&tm, h->ev[EV_FMT_BEGIN], h->ev[EV_FMT_END])); h->ring.ms_fmt += tm;
     return 0;
 }
-
-// ---- view -f bam (RUN_VIEW_BAM).  Per sub-batch: k_bam_len sizes the selected reads, the SAM scan gives their offsets, k_bam_write gathers
-// them behind the carried bytes of the open member, the member cut (k_bam_next .. k_bam_members) lists the members that close, k_bgzf_deflate
-// compresses them, and they go out through the text slots in pieces of whole members (k_bgzf_pack).  The open member's bytes move to `carry`.
-int bam_scan(bdepth* h, const uint32_t* len, uint32_t n, DevBuf& tiles, unsigned long long* off, unsigned long long* total) {
+// n lengths into 64-bit offsets and their sum at the device word *total: tile sums, k_text_scan over the tiles, then each tile's own scan
+int offset_scan(bdepth* h, const uint32_t* len, uint32_t n, DevBuf& tiles, unsigned long long* off, unsigned long long* total) {
     const uint32_t n_tiles = (n + SAM_SCAN_TILE - 1) / SAM_SCAN_TILE;
     const size_t toff_at = ((size_t)n_tiles * 4 + 7) / 8 * 8;
     CK(tiles.ensure(toff_at + (size_t)n_tiles * 8 + 8));
@@ -824,10 +768,95 @@ int bam_scan(bdepth* h, const uint32_t* len, uint32_t n, DevBuf& tiles, unsigned
     CK(cudaGetLastError()); h->st.gpu_launches += 3;
     return 0;
 }
-// Compress the nm members listed in vb.m_off / vb.m_len (offsets into stage) and hand them to the callback, in order.  ev[30] was recorded
-// by the caller where its GPU work began: that span is counted in the formatting time.
+// The n items at off (total bytes) through the ring, in pieces: write(first, last, slot) launches, on the main stream, the kernel that writes
+// items [first, last) into a slot.  The last piece is still pending on return (ring_flush hands it out).
+template <class Write> int ring_pieces(bdepth* h, const unsigned long long* off, uint32_t n, uint64_t total, Write&& write) {
+    auto& Q = h->ring; cudaStream_t sm = h->s_main;
+    const uint64_t piece = ring_piece(h);
+    const uint32_t n_cuts = (uint32_t)((total + piece - 1) / piece) + 1;
+    CK(Q.cut_r.ensure((size_t)n_cuts * 4)); CK(Q.cut_o.ensure((size_t)n_cuts * 8));
+    BD_LAUNCH((n_cuts + 255) / 256, 256, 0, sm, k_sam_cut)(off, n, total, piece, n_cuts, Q.cut_r.as<uint32_t>(), Q.cut_o.as<unsigned long long>());
+    CK(cudaGetLastError()); h->st.gpu_launches++;
+    std::vector<uint32_t> cr(n_cuts); std::vector<unsigned long long> co(n_cuts);
+    CK(cudaMemcpyAsync(cr.data(), Q.cut_r.p, (size_t)n_cuts * 4, cudaMemcpyDeviceToHost, sm)); CK(cudaMemcpyAsync(co.data(), Q.cut_o.p, (size_t)n_cuts * 8, cudaMemcpyDeviceToHost, sm));
+    CK(cudaStreamSynchronize(sm));
+    for (uint32_t j = 0; j + 1 < n_cuts; j++) {
+        const uint32_t i0 = cr[j], i1 = j + 2 == n_cuts ? n : cr[j + 1];
+        const uint64_t bytes = (j + 2 == n_cuts ? total : co[j + 1]) - co[j];
+        if (!bytes) continue;
+        const int s = Q.next;
+        int rc = ring_deliver(h, s); if (rc) return rc;      // the slot's previous piece must be consumed before reuse
+        CK(cudaEventRecord(h->ev[EV_RING_BEGIN + s], sm));
+        write(i0, i1, Q.slot[s].p);
+        CK(cudaGetLastError()); h->st.gpu_launches++;
+        CK(cudaEventRecord(h->ev[EV_RING_WRITTEN + s], sm));
+        CK(cudaStreamWaitEvent(h->s_d2h, h->ev[EV_RING_WRITTEN + s], 0));
+        CK(cudaMemcpyAsync(Q.host + (size_t)s * Q.cap, Q.slot[s].p, bytes, cudaMemcpyDeviceToHost, h->s_d2h));
+        CK(cudaEventRecord(h->ev[EV_RING_COPIED + s], h->s_d2h));
+        Q.pend[s] = true; Q.pend_len[s] = bytes; Q.next = s ^ 1;
+        rc = ring_deliver(h, s ^ 1); if (rc) return rc;     // hand out the previous piece while this one is in flight
+    }
+    return 0;
+}
+
+// ---- view's SAM lines (RUN_VIEW_TEXT).  Per sub-batch, while its records are still in the inflate buffer: k_sam_len measures the line of every
+// selected record, the offset scan turns the lengths into offsets, one small copy brings the total, the longest line and the error word down,
+// and the lines go out through the ring, each piece written by k_sam_write (a piece always holds whole lines, so a slot holds a piece plus the
+// longest line).  JSON records take k_json_len and k_json_write.
+const char* sam_err_msg(unsigned long long c) {
+    switch (c) {
+        case SAM_ERR_REF: return "a record's reference ID lies outside [-1, n_ref): no RNAME to print (the reference indexes its reference list out of bounds)";
+        case SAM_ERR_MATE_REF: return "a record's mate reference ID lies outside [-1, n_ref): no RNEXT to print (the reference indexes its reference list out of bounds)";
+        case SAM_ERR_TAG_TYPE: return "unknown tag type in a record's auxiliary data (UnknownTagTypeException)";
+        case SAM_ERR_B_TYPE: return "unknown element type of a B array in a record's auxiliary data (UnknownTagTypeException)";
+        case SAM_ERR_NO_NUL: return "a Z or H tag value without its terminating NUL";
+        default: return "a record's fields, a tag or a B array run past the record's block_size";
+    }
+}
+// view -v: k_view_valid over the sub-batch's R records, and vs (the run's selection) pointed at its statuses, refusals going to *err
+int launch_view_valid(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R, int64_t own_from, unsigned long long* err, ViewSel& vs) {
+    CK(h->vv.ensure(R));
+    BD_LAUNCH((unsigned)std::min<uint64_t>((R + VV_WARPS - 1) / VV_WARPS, 8192), VV_WARPS * 32, 0, h->s_main, k_view_valid)(soa, u0, R, own_from, h->vv.as<uint8_t>());
+    CK(cudaGetLastError()); h->st.gpu_launches++;
+    vs.vstat = h->vv.as<uint8_t>(); vs.verr = err;
+    return 0;
+}
+int view_text_sub(bdepth* h, const RecordSoA& soa, const uint8_t* u0, uint32_t R, int64_t own_from) {
+    auto& V = h->vt; cudaStream_t sm = h->s_main;
+    CK(V.len.ensure((size_t)R * 4)); CK(V.off.ensure((size_t)R * 8)); CK(V.ctl.ensure(32));
+    uint32_t* len = V.len.as<uint32_t>(); unsigned long long* off = V.off.as<unsigned long long>();
+    SamTab t = V.tab; t.ctl = V.ctl.as<unsigned long long>();
+    CK(cudaMemsetAsync(t.ctl, 0, 24, sm));
+    CK(cudaEventRecord(h->ev[EV_FMT_BEGIN], sm));
+    ViewSel vs = h->vsel;
+    if (h->view_valid) { int rc = launch_view_valid(h, soa, u0, R, own_from, t.ctl + 2, vs); if (rc) return rc; }      // refusals share the lines' error word
+    if (V.fmt == TEXT_JSON) BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_json_len)(soa, u0, R, own_from, vs, t, len);
+    else BD_LAUNCH((unsigned)std::min<uint64_t>((R + 7) / 8, 8192), 256, 0, sm, k_sam_len)(soa, u0, R, own_from, vs, t, len);
+    CK(cudaGetLastError()); h->st.gpu_launches++;
+    int rc = offset_scan(h, len, R, V.tiles, off, t.ctl); if (rc) return rc;
+    unsigned long long c[3]; rc = fmt_span_end(h, c, t.ctl, sizeof c); if (rc) return rc;
+    if (c[2]) return fail(h, BDEPTH_ERR_FORMAT, "%s", sam_err_msg(c[2]));
+    const uint64_t total = c[0], piece = ring_piece(h);
+    if (!total) return 0;
+    rc = ring_reserve(h, piece + c[1], piece + std::max<uint64_t>(c[1], piece)); if (rc) return rc;      // a slot holds a piece and its longest line
+    rc = ring_pieces(h, off, R, total, [&](uint32_t r0, uint32_t r1, void* slot) {
+        const unsigned grid = (unsigned)std::min<uint64_t>((r1 - r0 + 7) / 8, 8192);
+        if (V.fmt == TEXT_JSON) BD_LAUNCH(grid, 256, 0, sm, k_json_write)(soa.off, u0, r0, r1, len, off, t, (char*)slot);
+        else BD_LAUNCH(grid, 256, 0, sm, k_sam_write)(soa.off, u0, r0, r1, len, off, t, (char*)slot);
+    });
+    if (rc) return rc;
+    h->ring.issued += total;      // every line went to the D2H
+    return 0;
+}
+
+// ---- view -f bam (RUN_VIEW_BAM).  Per sub-batch: k_bam_len sizes the selected reads, the offset scan gives their offsets, k_bam_write gathers
+// them behind the carried bytes of the open member, the member cut (k_bam_next .. k_bam_members) lists the members that close, k_bgzf_deflate
+// compresses them, and they go out through the ring in pieces of whole members (k_bgzf_pack).  The open member's bytes move to `carry`.
+
+// Compress the nm members listed in vb.m_off / vb.m_len (offsets into stage) and hand them to the callback, in order.  EV_FMT_BEGIN was
+// recorded by the caller where its GPU work began: that span is counted in the formatting time.
 int bam_emit(bdepth* h, const uint8_t* stage, uint32_t nm) {
-    auto& B = h->vb; auto& V = h->vt; cudaStream_t sm = h->s_main;
+    auto& B = h->vb; cudaStream_t sm = h->s_main;
     CK(B.comp.ensure((size_t)nm * BGZF_SLOT)); CK(B.clen.ensure((size_t)nm * 4)); CK(B.coff.ensure((size_t)nm * 8 + 8)); CK(B.ctl.ensure(128));
     const uint32_t grid = std::min<uint32_t>(nm, (uint32_t)std::max(1, h->n_sm));
     CK(B.tok.ensure((size_t)grid * DF_THREADS * 256 * 4));
@@ -836,43 +865,13 @@ int bam_emit(bdepth* h, const uint8_t* stage, uint32_t nm) {
     CK(cudaGetLastError()); h->st.gpu_launches++;
     unsigned long long* tot_d = B.ctl.as<unsigned long long>() + 8;
     unsigned long long* coff = B.coff.as<unsigned long long>();
-    int rc = bam_scan(h, B.clen.as<uint32_t>(), nm, B.ctiles, coff, tot_d); if (rc) return rc;
-    CK(cudaEventRecord(h->ev[31], sm));
-    unsigned long long total = 0; CK(cudaMemcpyAsync(&total, tot_d, 8, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
-    { float tm = 0; CK(cudaEventElapsedTime(&tm, h->ev[30], h->ev[31])); V.ms_fmt += tm; }
-    const uint64_t piece = std::max<uint64_t>(1, std::min<uint64_t>(VIEW_TEXT_PIECE, h->batch_u));
-    if (piece + BGZF_SLOT > V.cap) {      // a slot holds a piece and one more member: grow both, after handing out what is pending in them
-        rc = view_text_flush(h); if (rc) return rc;
-        if (V.host) { cudaFreeHost(V.host); V.host = nullptr; }
-        V.cap = 0;
-        const size_t need = piece + BGZF_SLOT;
-        CK(cudaMallocHost((void**)&V.host, 2 * need)); CK(V.slot[0].ensure(need)); CK(V.slot[1].ensure(need));
-        V.cap = need;
-    }
-    const uint32_t n_cuts = (uint32_t)((total + piece - 1) / piece) + 1;
-    CK(V.cut_r.ensure((size_t)n_cuts * 4)); CK(V.cut_o.ensure((size_t)n_cuts * 8));
-    BD_LAUNCH((n_cuts + 255) / 256, 256, 0, sm, k_sam_cut)(coff, nm, total, piece, n_cuts, V.cut_r.as<uint32_t>(), V.cut_o.as<unsigned long long>());
-    CK(cudaGetLastError()); h->st.gpu_launches++;
-    std::vector<uint32_t> cr(n_cuts); std::vector<unsigned long long> co(n_cuts);
-    CK(cudaMemcpyAsync(cr.data(), V.cut_r.p, (size_t)n_cuts * 4, cudaMemcpyDeviceToHost, sm)); CK(cudaMemcpyAsync(co.data(), V.cut_o.p, (size_t)n_cuts * 8, cudaMemcpyDeviceToHost, sm));
-    CK(cudaStreamSynchronize(sm));
-    for (uint32_t j = 0; j + 1 < n_cuts; j++) {
-        const uint32_t m0 = cr[j], m1 = j + 2 == n_cuts ? nm : cr[j + 1];
-        const uint64_t bytes = (j + 2 == n_cuts ? total : co[j + 1]) - co[j];
-        if (!bytes) continue;
-        const int s = V.next;
-        rc = view_text_deliver(h, s); if (rc) return rc;
-        CK(cudaEventRecord(h->ev[28 + s], sm));
-        BD_LAUNCH(std::min<uint32_t>(m1 - m0, 4096), 256, 0, sm, k_bgzf_pack)(B.comp.as<uint8_t>(), B.clen.as<uint32_t>(), coff, m0, m1, V.slot[s].as<uint8_t>());
-        CK(cudaGetLastError()); h->st.gpu_launches++;
-        CK(cudaEventRecord(h->ev[24 + s], sm));
-        CK(cudaStreamWaitEvent(h->s_d2h, h->ev[24 + s], 0));
-        CK(cudaMemcpyAsync(V.host + (size_t)s * V.cap, V.slot[s].p, bytes, cudaMemcpyDeviceToHost, h->s_d2h));
-        CK(cudaEventRecord(h->ev[26 + s], h->s_d2h));
-        V.pend[s] = true; V.pend_len[s] = bytes; V.next = s ^ 1;
-        rc = view_text_deliver(h, s ^ 1); if (rc) return rc;
-    }
-    return 0;
+    int rc = offset_scan(h, B.clen.as<uint32_t>(), nm, B.ctiles, coff, tot_d); if (rc) return rc;
+    unsigned long long total = 0; rc = fmt_span_end(h, &total, tot_d, sizeof total); if (rc) return rc;
+    const uint64_t piece = ring_piece(h);
+    rc = ring_reserve(h, piece + BGZF_SLOT, piece + BGZF_SLOT); if (rc) return rc;      // a slot holds a piece and one more member
+    return ring_pieces(h, coff, nm, total, [&](uint32_t m0, uint32_t m1, void* slot) {
+        BD_LAUNCH(std::min<uint32_t>(m1 - m0, 4096), 256, 0, sm, k_bgzf_pack)(B.comp.as<uint8_t>(), B.clen.as<uint32_t>(), coff, m0, m1, (uint8_t*)slot);
+    });
 }
 // Members of BGZF_BLOCK bytes over n bytes at stage (the last one shorter): the header and reference list, and the last open member.
 int bam_emit_run(bdepth* h, const uint8_t* stage, uint64_t n) {
@@ -883,7 +882,7 @@ int bam_emit_run(bdepth* h, const uint8_t* stage, uint64_t n) {
     for (uint32_t k = 0; k < nm; k++) { mo[k] = (unsigned long long)k * BGZF_BLOCK; ml[k] = (uint32_t)std::min<uint64_t>(BGZF_BLOCK, n - mo[k]); }
     CK(B.m_off.ensure((size_t)nm * 8)); CK(B.m_len.ensure((size_t)nm * 4));
     CK(cudaMemcpy(B.m_off.p, mo.data(), (size_t)nm * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(B.m_len.p, ml.data(), (size_t)nm * 4, cudaMemcpyHostToDevice));
-    CK(cudaEventRecord(h->ev[30], h->s_main));
+    CK(cudaEventRecord(h->ev[EV_FMT_BEGIN], h->s_main));
     return bam_emit(h, stage, nm);
 }
 // ---- the record pipeline: one front end shared by every run mode (H2D, K1 inflate, the K2 record-chain walk with its host verification,
@@ -1382,17 +1381,17 @@ int consume_view_bam(Pipe& P, const SubBatch& s) {
     unsigned long long* ctl = B.ctl.as<unsigned long long>();      // [0] bytes gathered, [2] error, [3] P', [4] cur', [5] members, [7] s0
     uint32_t* len = B.len.as<uint32_t>(); unsigned long long* off = B.off.as<unsigned long long>();
     CK(cudaMemsetAsync(ctl, 0, 64, sm));
-    CK(cudaEventRecord(h->ev[30], sm));
+    CK(cudaEventRecord(h->ev[EV_FMT_BEGIN], sm));
     ViewSel vs = h->vsel;
     if (h->view_valid) { int rc = launch_view_valid(h, s.soa, s.u0, R, INT64_MIN, ctl + 2, vs); if (rc) return rc; }
     BD_LAUNCH((R + 255) / 256, 256, 0, sm, k_bam_len)(s.soa, s.u0, R, INT64_MIN, vs, (uint32_t)h->hdr.ref_len.size(), ctl + 2, len);
     CK(cudaGetLastError()); h->st.gpu_launches++;
-    int rc = bam_scan(h, len, R, B.tiles, off, ctl); if (rc) return rc;
+    int rc = offset_scan(h, len, R, B.tiles, off, ctl); if (rc) return rc;
     unsigned long long c[3]; CK(cudaMemcpyAsync(c, ctl, 24, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
     if (c[2]) return fail(h, BDEPTH_ERR_FORMAT, "%s", c[2] == BAM_ERR_REF ? "Read reference ID is out of range" : sam_err_msg(c[2]));
     const unsigned long long total = c[0];
-    if (!total) { CK(cudaEventRecord(h->ev[31], sm)); CK(cudaStreamSynchronize(sm)); float tm = 0; CK(cudaEventElapsedTime(&tm, h->ev[30], h->ev[31])); h->vt.ms_fmt += tm; return 0; }
-    h->vt.issued += total;      // (records that joined the open member are output: a restart of the run would repeat them)
+    if (!total) return fmt_span_end(h);
+    h->ring.issued += total;      // (records that joined the open member are output: a restart of the run would repeat them)
     CK(B.stage.ensure(B.P + total + 16));
     uint8_t* stage = B.stage.as<uint8_t>();
     if (B.P) CK(cudaMemcpyAsync(stage, B.carry.p, B.P, cudaMemcpyDeviceToDevice, sm));
@@ -1411,7 +1410,7 @@ int consume_view_bam(Pipe& P, const SubBatch& s) {
     for (uint32_t k = K; k-- > 0;) BD_LAUNCH(g, 256, 0, sm, k_bam_mark)(J + (size_t)k * (R + 1), mark, R);
     BD_LAUNCH(g, 256, 0, sm, k_bam_members<false>)(off, R, total, J, mark, s0, B.P, B.cur, B.cnt.as<uint32_t>(), nullptr, nullptr, nullptr, nullptr);
     CK(cudaGetLastError()); h->st.gpu_launches += 2 * K + 3;
-    rc = bam_scan(h, B.cnt.as<uint32_t>(), R + 1, B.tiles, B.base.as<unsigned long long>(), ctl + 5); if (rc) return rc;
+    rc = offset_scan(h, B.cnt.as<uint32_t>(), R + 1, B.tiles, B.base.as<unsigned long long>(), ctl + 5); if (rc) return rc;
     const unsigned long long max_m = 3 * (B.P + total) / BGZF_BLOCK + 4;
     CK(B.m_off.ensure(max_m * 8)); CK(B.m_len.ensure(max_m * 4));
     BD_LAUNCH(g, 256, 0, sm, k_bam_members<true>)(off, R, total, J, mark, s0, B.P, B.cur, B.cnt.as<uint32_t>(), B.base.as<unsigned long long>(),
@@ -1419,8 +1418,7 @@ int consume_view_bam(Pipe& P, const SubBatch& s) {
     CK(cudaGetLastError()); h->st.gpu_launches++;
     CK(cudaMemcpyAsync(c, ctl + 3, 24, cudaMemcpyDeviceToHost, sm)); CK(cudaStreamSynchronize(sm));
     const uint32_t P2 = (uint32_t)c[0]; const unsigned long long cur2 = c[1]; const uint32_t nm = (uint32_t)c[2];
-    if (nm) { rc = bam_emit(h, stage, nm); if (rc) return rc; }
-    else { CK(cudaEventRecord(h->ev[31], sm)); CK(cudaStreamSynchronize(sm)); float tm = 0; CK(cudaEventElapsedTime(&tm, h->ev[30], h->ev[31])); h->vt.ms_fmt += tm; }
+    rc = nm ? bam_emit(h, stage, nm) : fmt_span_end(h); if (rc) return rc;
     if (P2) { CK(B.carry.ensure(BGZF_BLOCK)); CK(cudaMemcpyAsync(B.carry.p, stage + B.P + total - P2, P2, cudaMemcpyDeviceToDevice, sm)); }
     B.P = P2; B.cur = cur2;
     return 0;
@@ -1434,7 +1432,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
     auto t_host0 = std::chrono::steady_clock::now();
     bdepth_stats& st = h->st; st = bdepth_stats{};
     const ModeNeeds& need = MODE_NEEDS[mode]; Pipe P{h, mode, ro, em};
-    h->vt.issued = 0; h->vt.ms_fmt = h->vt.ms_d2h = 0;      // every mode: a sparse restart below refuses a run that has handed out SAM lines (vt.issued)
+    h->ring.issued = 0; h->ring.ms_fmt = h->ring.ms_d2h = 0;      // every mode: a sparse restart below refuses a run that has handed out output (ring.issued)
     const bool sparse = P.sparse = need.may_stage_sparse && plan_sparse(h);      // (view: bdepth_run_view_count / _text has put its own regions there)
     h->coll_pending = (h->world <= 1 || !h->comm || need.owes == Owed::NOTHING) ? Owed::NOTHING : sparse ? Owed::SPARSE_DECISION : need.owes;      // a sparse query first owes the decision
     if (!sparse) { rc = prepare_shard(h); if (rc) return rc; }      // the plain path needs the whole file's member table (a lazily opened handle frames it now)
@@ -1559,7 +1557,7 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             // the index does not describe this file (the reference only checks that one exists): plain pass instead.
             // On several ranks that decision has to be taken by all of them together (below, after the batches):
             // a rank falling back on its own would leave the union of the ranks' records no partition of the file.
-            if (h->world == 1) { if (h->vt.issued) return refuse_index_after_text(h); h->sparse_ok = false; CK(cudaDeviceSynchronize()); return RC_RESTART; }
+            if (h->world == 1) { if (h->ring.issued) return refuse_index_after_text(h); h->sparse_ok = false; CK(cudaDeviceSynchronize()); return RC_RESTART; }
             sparse_bad = true; break;
         }
         rc = decode_records(P, s, snb); if (rc) return rc;
@@ -1615,8 +1613,8 @@ int run_pipeline_body(bdepth* h, RunMode mode, RunOut* ro, Emitter* em) {
             }
             rc = finish_census(h, need.owes); if (rc) return rc; st.ms_reduce = P.ms_census; break;
         case RUN_VIEW_TEXT: case RUN_VIEW_BAM:
-            rc = view_text_flush(h); if (rc) return rc;      // the last piece, before the ranks learn that this one is complete
-            st.ms_d2h = h->vt.ms_d2h; rc = finish_census(h, need.owes); if (rc) return rc; st.ms_reduce = h->vt.ms_fmt;
+            rc = ring_flush(h); if (rc) return rc;      // the last piece, before the ranks learn that this one is complete
+            st.ms_d2h = h->ring.ms_d2h; rc = finish_census(h, need.owes); if (rc) return rc; st.ms_reduce = h->ring.ms_fmt;
             break;
         case RUN_FULL:
             st.positions = h->hdr.total_len;
@@ -1668,7 +1666,8 @@ void index_extent(const bdepth* h, uint64_t& lo, uint64_t& hi) {
 void add_stats(bdepth_stats& t, const bdepth_stats& s) {
     t.file_bytes += s.file_bytes; t.n_blocks += s.n_blocks; t.cdata_bytes += s.cdata_bytes; t.inflated_bytes += s.inflated_bytes; t.n_records += s.n_records; t.n_records_pass += s.n_records_pass;
     t.n_cigar_ops += s.n_cigar_ops; t.seq_bytes += s.seq_bytes; t.long_reads += s.long_reads; t.chain_fixups += s.chain_fixups; t.gpu_launches += s.gpu_launches; t.n_batches += s.n_batches;
-    t.ms_h2d += s.ms_h2d; t.ms_inflate += s.ms_inflate; t.ms_scan += s.ms_scan; t.ms_coverage += s.ms_coverage; t.ms_span_device += s.ms_span_device; t.host_wall_ms += s.host_wall_ms;
+    t.ms_h2d += s.ms_h2d; t.ms_inflate += s.ms_inflate; t.ms_scan += s.ms_scan; t.ms_coverage += s.ms_coverage; t.ms_reduce += s.ms_reduce; t.ms_d2h += s.ms_d2h;
+    t.ms_span_device += s.ms_span_device; t.host_wall_ms += s.host_wall_ms;
 }
 // The pipeline over every input of the handle, into one set of counters (RUN_FULL).  One input: run_pipeline as it is.
 int run_all_inputs(bdepth* h, Emitter* em = nullptr) {
@@ -1809,7 +1808,8 @@ void bdepth_close(bdepth_t* h) {
     { auto& X = h->ix; X.lin.release(); X.lin_len.release(); X.lin_base.release(); X.lin_cap.release(); X.n_mapped.release(); X.n_unmapped.release(); X.carry.release(); X.ctl.release(); X.runs.release(); X.excs.release(); }
     h->m_hash.release(); h->m_flag.release(); h->m_ctl.release(); h->fprog_d.release();
     h->vc.release(); h->vc_reg.release(); h->vc_prog.release(); h->vv.release();
-    { auto& V = h->vt; V.names.release(); V.len.release(); V.off.release(); V.tiles.release(); V.ctl.release(); V.cut_r.release(); V.cut_o.release(); V.slot[0].release(); V.slot[1].release(); if (V.host) cudaFreeHost(V.host); V.host = nullptr; V.cap = 0; }
+    { auto& V = h->vt; V.names.release(); V.len.release(); V.off.release(); V.tiles.release(); V.ctl.release(); }
+    { auto& Q = h->ring; Q.cut_r.release(); Q.cut_o.release(); Q.slot[0].release(); Q.slot[1].release(); if (Q.host) cudaFreeHost(Q.host); Q.host = nullptr; Q.cap = 0; }
     if (h->comm) { nccl().CommDestroy(h->comm); h->comm = nullptr; }
     if (h->pinned) cudaFreeHost(h->pinned);
     h->hs.release();
@@ -2423,13 +2423,17 @@ int view_setup(bdepth* h, const bdepth_view_opts* o, const bdepth_region* regs, 
 // ReadCounter over view_main's selection (sambamba/view.d:265-368): K1 + K2 as in every run, then k_view_count per sub-batch.  Regions on a
 // coordinate-sorted file with a usable index stage only their BAI chunks (plan_sparse, with the view's regions in place of the handle's for the
 // duration of the run); otherwise every record of the file is scanned.  The handle's depth settings are not used and stay as they were.
-int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* o, uint64_t* count) {
+static int view_args(bdepth_t* h, const bdepth_view_opts* o, bool have_out) {      // the checks every view entry point opens with
     if (!h) return BDEPTH_ERR_ARG;
-    if (!o || !count || (o->n_regions && !o->regions)) return fail(h, BDEPTH_ERR_ARG, "null argument");
+    if (!o || !have_out || (o->n_regions && !o->regions)) return fail(h, BDEPTH_ERR_ARG, "null argument");
     if (o->regions_from < BDEPTH_VIEW_ALL || o->regions_from > BDEPTH_VIEW_POSITIONAL) return fail(h, BDEPTH_ERR_ARG, "regions_from: %d", o->regions_from);
     if (!h->extra.empty()) return fail(h, BDEPTH_ERR_ARG, "view reads one BAM file: this handle has several inputs (bdepth_add_input)");
+    return 0;
+}
+int bdepth_run_view_count(bdepth_t* h, const bdepth_view_opts* o, uint64_t* count) {
+    int rc = view_args(h, o, count != nullptr); if (rc) return rc;
     std::vector<bdepth_region> plan; bool empty = false;
-    int rc = view_setup(h, o, o->regions, o->n_regions, o->n_unmapped, plan, &empty); if (rc) return rc;
+    rc = view_setup(h, o, o->regions, o->n_regions, o->n_unmapped, plan, &empty); if (rc) return rc;
     if (empty) { *count = 0; h->st = bdepth_stats{}; return 0; }
     std::swap(h->regions, plan);
     rc = run_pipeline(h, RUN_VIEW_COUNT, nullptr);
@@ -2453,17 +2457,14 @@ static std::string json_quote(const std::string& s) {      // writeStringJson (f
     return q + "\"";
 }
 static int run_view_lines(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb cb, void* user, TextFormat fmt, const char* header_text = nullptr, size_t header_len = 0) {
-    if (!h) return BDEPTH_ERR_ARG;
-    if (!o || (o->n_regions && !o->regions)) return fail(h, BDEPTH_ERR_ARG, "null argument");
-    if (o->regions_from < BDEPTH_VIEW_ALL || o->regions_from > BDEPTH_VIEW_POSITIONAL) return fail(h, BDEPTH_ERR_ARG, "regions_from: %d", o->regions_from);
-    if (!h->extra.empty()) return fail(h, BDEPTH_ERR_ARG, "view reads one BAM file: this handle has several inputs (bdepth_add_input)");
+    int rc = view_args(h, o, true); if (rc) return rc;
     if (o->n_unmapped) return fail(h, BDEPTH_ERR_ARG, "n_unmapped: give each '*' in its place in the region list (ref_id BDEPTH_VIEW_UNMAPPED)");
     const bool positional = o->regions_from == BDEPTH_VIEW_POSITIONAL;
     if (positional && h->world > 1) return fail(h, BDEPTH_ERR_ARG, "positional regions on several ranks: each region's lines would be split over the ranks (run them on one GPU)");
     if (fmt == TEXT_BAM && h->world > 1) return fail(h, BDEPTH_ERR_ARG, "view -f bam on several ranks: the member cut of a rank starts from the previous rank's state (run it on one GPU)");
     const size_t nref = h->hdr.ref_len.size();
-    int rc = init_device(h); if (rc) return rc;
-    auto& V = h->vt;
+    rc = init_device(h); if (rc) return rc;
+    auto& V = h->vt; auto& Q = h->ring;
     {   // the reference names, once per call: offsets, then the names
         std::vector<uint32_t> noff(nref + 1, 0); std::string all;
         for (size_t r = 0; r < nref; r++) { noff[r] = (uint32_t)all.size(); all += fmt == TEXT_JSON ? json_quote(h->hdr.ref_names[r]) : h->hdr.ref_names[r]; }
@@ -2473,7 +2474,7 @@ static int run_view_lines(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb
         if (!all.empty()) CK(cudaMemcpy(V.names.as<uint8_t>() + (nref + 1) * 4, all.data(), all.size(), cudaMemcpyHostToDevice));
         V.tab = SamTab{(const char*)(V.names.as<uint8_t>() + (nref + 1) * 4), V.names.as<uint32_t>(), (int32_t)nref, nullptr};
     }
-    V.cb = cb; V.user = user; V.pend[0] = V.pend[1] = false; V.next = 0; V.fmt = fmt; V.ms_fmt = V.ms_d2h = 0;
+    V.fmt = fmt; Q.cb = cb; Q.user = user; Q.pend[0] = Q.pend[1] = false; Q.next = 0; Q.ms_fmt = Q.ms_d2h = 0;
     bool header_out = fmt != TEXT_BAM;
     auto bam_header = [&]() -> int {      // BamWriter: BAM_MAGIC, writeSamHeader, writeReferenceSequenceInfo, flushCurrentBlock
         std::string b("BAM\1", 4);
@@ -2495,10 +2496,7 @@ static int run_view_lines(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb
         r = run_pipeline(h, fmt == TEXT_BAM ? RUN_VIEW_BAM : RUN_VIEW_TEXT, nullptr);
         std::swap(h->regions, plan);
         if (r) return r;
-        const bdepth_stats& s = h->st;
-        acc.file_bytes += s.file_bytes; acc.n_blocks += s.n_blocks; acc.n_records += s.n_records; acc.n_batches += s.n_batches; acc.gpu_launches += s.gpu_launches;
-        acc.ms_h2d += s.ms_h2d; acc.ms_inflate += s.ms_inflate; acc.ms_scan += s.ms_scan; acc.ms_reduce += s.ms_reduce; acc.ms_d2h += s.ms_d2h;
-        acc.ms_span_device += s.ms_span_device; acc.host_wall_ms += s.host_wall_ms;
+        add_stats(acc, h->st);
         return 0;
     };
     bdepth_stats acc{};
@@ -2521,10 +2519,10 @@ static int run_view_lines(bdepth_t* h, const bdepth_view_opts* o, bdepth_text_cb
         }
     }
     if (fmt == TEXT_BAM) {      // the open member, then BGZF_EOF (BgzfOutputStream.close)
-        V.ms_fmt = 0; V.ms_d2h = 0;
+        Q.ms_fmt = 0; Q.ms_d2h = 0;
         if (h->vb.P) { rc = bam_emit_run(h, h->vb.carry.as<uint8_t>(), h->vb.P); if (rc) return rc; h->vb.P = 0; }
-        rc = view_text_flush(h); if (rc) return rc;
-        acc.ms_reduce += V.ms_fmt; acc.ms_d2h += V.ms_d2h;
+        rc = ring_flush(h); if (rc) return rc;
+        acc.ms_reduce += Q.ms_fmt; acc.ms_d2h += Q.ms_d2h;
         static const uint8_t BGZF_EOF[28] = {31, 139, 8, 4, 0, 0, 0, 0, 0, 255, 6, 0, 66, 67, 2, 0, 27, 0, 3, 0, 0, 0, 0, 0, 0, 0, 0, 0};
         if (cb && cb(user, (const char*)BGZF_EOF, sizeof BGZF_EOF)) return fail(h, BDEPTH_ERR_CALLBACK, "text callback aborted");
     }
